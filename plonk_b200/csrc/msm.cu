@@ -15,9 +15,10 @@
 //     turns it into bucket offsets; (3) (point,sign) references are scattered into bucket order;
 //     (4) bucket accumulation: SPLIT threads per bucket add their share of the bucket's points
 //     with XYZZ mixed additions (8M + 2S each) - this is where the G1 adds of the workload are;
-//     (5) bucket reduction sum_b (b+1) B_b: running sums over groups of 8 buckets, then 8-ary
-//     trees of the group sums split by the bits of the group index; the last few dozen additions
-//     (Horner over those bits) and the single inversion for the affine result run on the host.
+//     (5) bucket reduction sum_b (b+1) B_b: row and column sums of the buckets laid out 8 to a row,
+//     then plain sums of the row sums split by the digits of the row index; the last few dozen
+//     additions (Horner over those digits) and the single inversion for the affine result run on
+//     the host.
 //   * `batch` scalar vectors against the same key are processed by the same launches
 //     (Prover::commit_polynomials commits 4 polynomials at once, src/compiler/prover.rs:187-210).
 #include <algorithm>
@@ -38,15 +39,17 @@ struct pb200_srs {
 namespace pb {
 
 static constexpr int kGroup = 8;
-static constexpr unsigned kClassChunk = 512;  // members of a class summed by one warp
 // Over-long buckets leave the one-thread-group-per-bucket kernel: they are cut into chunks of kHeavyChunk
 // entries, one warp per chunk, and the chunk sums are added per bucket afterwards.  "Over-long" is decided
 // on the device from the MSM's actual load (k_msm_scan): more than max(kHeavyMin, kHeavyFactor x the average
 // bucket) entries.  A dense MSM (uniform scalars, average 32..64) never has such a bucket; a sparse one (the
 // wire VALUES of a circuit: average 2, a tail of buckets with dozens to tens of thousands of entries) sends
 // its tail there, so that no lane of k_msm_accumulate walks more than a few dozen entries.
+// A warp's chunk is 8 entries per lane (kHeavyChunk) when the MSM is alone on the GPU, and 32 per lane
+// (kHeavyChunkWide) when other proofs keep the machine busy: the 5-level shuffle tree that ends every chunk
+// costs 5 full additions per lane, 60 % extra work on 8 mixed additions and 15 % on 32.
 static constexpr unsigned kHeavyMin = 32, kHeavyFactor = 4;
-static constexpr unsigned kHeavyChunk = 256;
+static constexpr unsigned kHeavyChunk = 256, kHeavyChunkWide = 1024;
 
 PB_D G1Affine ld_affine(const uint4* p, size_t i) {
   const uint4* q = p + 6 * i;
@@ -293,7 +296,8 @@ __global__ void k_msm_digits(const uint4* scalars, size_t n, size_t stride, int 
 // clipped size), so that the threads of a warp in k_msm_accumulate get buckets of near-equal length
 // and the warp does not idle on its longest lane.
 __global__ void __launch_bounds__(1024) k_msm_scan(const unsigned* counts, unsigned* offsets, unsigned* order, unsigned* n_heavy,
-                                                   unsigned* heavy_pre, unsigned* max_len, unsigned nb, int size_shift) {
+                                                   unsigned* heavy_pre, unsigned* max_len, unsigned nb, int size_shift,
+                                                   unsigned heavy_chunk) {
   __shared__ unsigned sums[1024];
   __shared__ unsigned bins[1024];
   __shared__ unsigned s_nh, s_total, s_thr_units, s_max;
@@ -361,13 +365,13 @@ __global__ void __launch_bounds__(1024) k_msm_scan(const unsigned* counts, unsig
     ord[pos] = k;
   }
   __syncthreads();  // ord[0 .. n_heavy) is complete (written by this CTA)
-  // heavy_pre[h] = number of kHeavyChunk-entry chunks of the heavy buckets before the h-th one
+  // heavy_pre[h] = number of heavy_chunk-entry chunks of the heavy buckets before the h-th one
   const unsigned nh = s_nh;
   unsigned* hp = heavy_pre + (size_t)b * (nb + 1);
   const unsigned per = (nh + 1023u) / 1024u;
   const unsigned h_lo = min(nh, tid * per), h_hi = min(nh, h_lo + per);
   unsigned c = 0;
-  for (unsigned h = h_lo; h < h_hi; h++) c += (cnt[ord[h]] + kHeavyChunk - 1) / kHeavyChunk;
+  for (unsigned h = h_lo; h < h_hi; h++) c += (cnt[ord[h]] + heavy_chunk - 1) / heavy_chunk;
   sums[tid] = c;
   __syncthreads();
   for (unsigned d = 1; d < 1024; d <<= 1) {
@@ -379,7 +383,7 @@ __global__ void __launch_bounds__(1024) k_msm_scan(const unsigned* counts, unsig
   unsigned run2 = sums[tid] - c;
   for (unsigned h = h_lo; h < h_hi; h++) {
     hp[h] = run2;
-    run2 += (cnt[ord[h]] + kHeavyChunk - 1) / kHeavyChunk;
+    run2 += (cnt[ord[h]] + heavy_chunk - 1) / heavy_chunk;
   }
   if (tid == 1023) hp[nh] = sums[1023];
 }
@@ -470,12 +474,13 @@ PB_D G1Xyzz warp_sum(G1Xyzz v) {
 
 // Heavy buckets (skewed scalars: many equal coefficients, 0/1 vectors, the wire VALUES of a circuit, whose
 // small entries pile tens of thousands of points onto digits 1, 2, 3 of the lowest window): the chunks of
-// all heavy buckets form one work list, a warp per chunk of kHeavyChunk entries (8 mixed additions per lane
-// and a shuffle tree), so a 30 000-entry bucket is spread over 118 warps instead of being walked by one CTA.
+// all heavy buckets form one work list, a warp per chunk of heavy_chunk entries (8 or 32 mixed additions per
+// lane and a shuffle tree), so a 30 000-entry bucket is spread over 30..118 warps instead of being walked by one CTA.
 // With uniformly random scalars there is no heavy bucket and the warps exit at once.
 __global__ void __launch_bounds__(128) k_msm_heavy_chunks(const uint4* table, const unsigned* sorted, const unsigned* offsets,
                                                           const unsigned* order, const unsigned* n_heavy, const unsigned* heavy_pre,
-                                                          unsigned nb, size_t cap, size_t part_cap, uint4* partials) {
+                                                          unsigned nb, unsigned heavy_chunk, size_t cap, size_t part_cap,
+                                                          uint4* partials) {
   const unsigned b = blockIdx.y;
   const unsigned nh = n_heavy[b];
   if (nh == 0) return;
@@ -492,7 +497,7 @@ __global__ void __launch_bounds__(128) k_msm_heavy_chunks(const uint4* table, co
       if (hp[mid] <= v) lo = mid; else hi = mid;
     }
     const unsigned bucket = ord[lo];
-    const unsigned start = off[bucket] + (v - hp[lo]) * kHeavyChunk, end = min(off[bucket + 1], start + kHeavyChunk);
+    const unsigned start = off[bucket] + (v - hp[lo]) * heavy_chunk, end = min(off[bucket + 1], start + heavy_chunk);
     G1Xyzz acc = G1Xyzz::identity();
     for (unsigned k = start + lane; k < end; k += 32) {
       const unsigned e = __ldg(src + k);
@@ -934,110 +939,134 @@ __global__ void __launch_bounds__(kAffThreads, 4) k_msm_affine_back(AffRound a) 
 }
 
 // ---------------------------------------------------------------------------------------------
-// Bucket reduction  R = sum_b (b + 1) B_b.  A single GPU thread needs ~15 us per dependent group
-// addition (14 carry-chained Fp products), so the reduction is organised to be work-efficient first
-// (it shares the SMs with other proofs' accumulation kernels) and shallow second:
-//   A. k_msm_groups: one thread per group of g = kGroup consecutive buckets, running sums:
-//        S_G = sum_j B[gG + j],  A_G = sum_j (j + 1) B[gG + j]          => R = sum A_G + g sum G S_G
-//   B. k_msm_group_classes: the group index G is cut into digits of <= 4 bits; class (j, v) is the
-//      plain sum of S_G over the groups whose digit j equals v; further classes hold partial plain
-//      sums of A_G.  One warp per class: 8..16 serial additions per lane + a 5-level shuffle tree.
-//   C. k_msm_final: one warp per digit turns its 16 class sums into D_j = sum_v v C_{j,v} (suffix
-//      scan + reduce); one more warp adds the A partials.  The host finishes with a Horner over
-//      the digits (a dozen doublings, ~10 us) and the affine normalisation.
+// Bucket reduction  R = sum_b (b + 1) B_b.  A lone warp needs ~10 us per dependent full addition (a dozen
+// carry-chained Fp products), and a reduction launch holds its registers for as long as its longest thread
+// runs, so the reduction is built wide and shallow at about the work of the old running-sum scheme.  Write
+// the bucket index as b = g G + j (g = kGroup buckets per row G, column j < g):
+//        R = sum_j (j + 1) T_j + g sum_G G S_G,   T_j = sum_G B[gG + j],   S_G = sum_j B[gG + j]
+//   A. k_msm_rows_cols: one thread per row sums its g buckets (S_G); one thread per run of kColRun rows of
+//      one column sums that piece of the column (partial T_j).  g - 1 = 7 serial additions per thread.
+//   B. k_msm_lists: the group index G is cut into digits of <= 4 bits; class (j, v) is the plain sum of S_G
+//      over the groups whose digit j equals v; column list j is the sum of the partials of column j.  One
+//      warp per (list, chunk of kListChunk members): 8 serial additions per lane + a 5-level shuffle tree.
+//      Lists of more than kFinalChunks chunks (windows of 20 bits) have their chunk sums added by one more
+//      warp tree per list (k_msm_fold).
+//   C. k_msm_final: one warp per digit turns its 16 class sums into D_j = sum_v v C_{j,v} (suffix scan +
+//      reduce); one more warp turns the g column sums into sum_j (j + 1) T_j the same way.  The host finishes
+//      with a Horner over the digits (a dozen doublings, ~10 us) and the affine normalisation.
+// For c = 16: 2^12 rows, 2^12 column partials, 48 classes of 256 members, 8 columns of 512 partials - about
+// 2.25 * 2^15 full additions, at most 7 + (7 + 5) + (1 + 4 + 4) = 28 of them dependent (38 for the running-sum
+// scheme it replaces), over 8192 threads per MSM in the widest launch (4096 before).
 // ---------------------------------------------------------------------------------------------
+static constexpr unsigned kColRun = 8;        // rows per partial column sum
+static constexpr unsigned kListChunk = 256;   // members of a list summed by one warp
+static constexpr unsigned kFinalChunks = 4;   // chunk sums per list that k_msm_final adds serially
+
 struct DigitPlan {
   int ndig;
   int shift[8];
   int bits[8];
   int first_class[8];  // prefix sum of 2^bits
   int n_digit_classes;
-  int n_a_classes;     // partial sums of A_G, 256 groups each
-  int nclasses;
+  int n_columns;       // g: column lists after the digit classes
+  int nlists;
 };
 
 template <bool AFFINE>
-__global__ void __launch_bounds__(64) k_msm_groups(const uint4* sums, unsigned nb, int g, uint4* S, uint4* A) {
-  const unsigned G = blockIdx.x * blockDim.x + threadIdx.x;
-  const unsigned n_groups = nb / g;
-  if (G >= n_groups) return;
-  const unsigned b = blockIdx.y;
-  G1Xyzz run = G1Xyzz::identity(), acc = G1Xyzz::identity();
-  for (int j = g - 1; j >= 0; j--) {
-    if (AFFINE) {  // bucket sums left by the batched-affine rounds: a mixed addition
-      const G1Affine q = ld_affine(sums, (size_t)b * nb + (size_t)G * g + j);
-      if (!q.is_inf()) xyzz_madd(run, q.x, q.y);
-    } else {
-      G1Xyzz q = ld_xyzz(sums, (size_t)b * nb + (size_t)G * g + j);
-      xyzz_add(run, q);
-    }
-    xyzz_add(acc, run);
+PB_D void add_bucket(G1Xyzz& acc, const uint4* sums, size_t i) {
+  if (AFFINE) {  // bucket sums left by the batched-affine rounds: a mixed addition
+    const G1Affine q = ld_affine(sums, i);
+    if (!q.is_inf()) xyzz_madd(acc, q.x, q.y);
+  } else {
+    xyzz_add(acc, ld_xyzz(sums, i));
   }
-  st_xyzz(S, (size_t)b * n_groups + G, run);
-  st_xyzz(A, (size_t)b * n_groups + G, acc);
 }
 
-// One warp per (class, chunk of kClassChunk members); 4 warps per CTA.  out is [batch][nclasses][chunks].
-__global__ void __launch_bounds__(128) k_msm_group_classes(const uint4* S, const uint4* A, unsigned n_groups,
-                                                           DigitPlan plan, unsigned chunks, uint4* out) {
-  const int cls = blockIdx.x * 4 + (threadIdx.x >> 5);
+// Threads [0, n_groups) of a batch entry: row sums S ([batch][n_groups]); threads [n_groups, n_groups + nb / col_run):
+// partial column sums P ([batch][g][n_groups / col_run]).
+template <bool AFFINE>
+__global__ void __launch_bounds__(64) k_msm_rows_cols(const uint4* sums, unsigned nb, unsigned g, unsigned col_run, uint4* S, uint4* P) {
+  const unsigned t = blockIdx.x * blockDim.x + threadIdx.x;
+  const unsigned n_groups = nb / g, n_parts = n_groups / col_run;
+  const unsigned b = blockIdx.y;
+  const size_t base = (size_t)b * nb;
+  G1Xyzz acc = G1Xyzz::identity();
+  if (t < n_groups) {
+    for (unsigned j = 0; j < g; j++) add_bucket<AFFINE>(acc, sums, base + (size_t)t * g + j);
+    st_xyzz(S, (size_t)b * n_groups + t, acc);
+  } else if (t < n_groups + g * n_parts) {
+    const unsigned u = t - n_groups, j = u / n_parts, part = u % n_parts;
+    for (unsigned k = 0; k < col_run; k++) add_bucket<AFFINE>(acc, sums, base + (size_t)(part * col_run + k) * g + j);
+    st_xyzz(P, ((size_t)b * g + j) * n_parts + part, acc);
+  }
+}
+
+// One warp per (list, chunk of kListChunk members); 4 warps per CTA.  out is [batch][nlists][chunks].
+__global__ void __launch_bounds__(128) k_msm_lists(const uint4* S, const uint4* P, unsigned n_groups, unsigned n_parts,
+                                                   DigitPlan plan, unsigned chunks, uint4* out) {
+  const int list = blockIdx.x * 4 + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   const unsigned b = blockIdx.y, chunk = blockIdx.z;
-  if (cls >= plan.nclasses) return;
+  if (list >= plan.nlists) return;
   G1Xyzz acc = G1Xyzz::identity();
-  if (cls < plan.n_digit_classes) {
+  if (list < plan.n_digit_classes) {
     int j = 0;
-    while (j + 1 < plan.ndig && cls >= plan.first_class[j + 1]) j++;
-    const unsigned v = cls - plan.first_class[j];
+    while (j + 1 < plan.ndig && list >= plan.first_class[j + 1]) j++;
+    const unsigned v = list - plan.first_class[j];
     const int sh_j = plan.shift[j], bits_j = plan.bits[j];
     const unsigned count = n_groups >> bits_j;
-    for (unsigned idx = chunk * kClassChunk + lane; idx < min(count, (chunk + 1) * kClassChunk); idx += 32) {
+    for (unsigned idx = chunk * kListChunk + lane; idx < min(count, (chunk + 1) * kListChunk); idx += 32) {
       const unsigned G = ((idx >> sh_j) << (sh_j + bits_j)) | (v << sh_j) | (idx & ((1u << sh_j) - 1u));
-      G1Xyzz q = ld_xyzz(S, (size_t)b * n_groups + G);
-      xyzz_add(acc, q);
+      xyzz_add(acc, ld_xyzz(S, (size_t)b * n_groups + G));
     }
-  } else if (chunk == 0) {
-    const unsigned first = (unsigned)(cls - plan.n_digit_classes) * 256u;
-    for (unsigned G = first + lane; G < min(n_groups, first + 256u); G += 32) {
-      G1Xyzz q = ld_xyzz(A, (size_t)b * n_groups + G);
-      xyzz_add(acc, q);
-    }
+  } else {
+    const size_t col = (size_t)b * plan.n_columns + (list - plan.n_digit_classes);
+    for (unsigned idx = chunk * kListChunk + lane; idx < min(n_parts, (chunk + 1) * kListChunk); idx += 32)
+      xyzz_add(acc, ld_xyzz(P, col * n_parts + idx));
   }
   acc = warp_sum(acc);
-  if (lane == 0) st_xyzz(out, ((size_t)b * plan.nclasses + cls) * chunks + chunk, acc);
+  if (lane == 0) st_xyzz(out, ((size_t)b * plan.nlists + list) * chunks + chunk, acc);
 }
 
-// out is [batch][ndig + 1]: D_0 .. D_{ndig-1}, then the sum of all A_G.
-__global__ void __launch_bounds__(256) k_msm_final(const uint4* classes, DigitPlan plan, unsigned chunks, uint4* out) {
-  const int lane = threadIdx.x & 31, j = threadIdx.x >> 5;
-  const unsigned b = blockIdx.x;
-  if (j < plan.ndig) {
-    const int nv = 1 << plan.bits[j];
-    G1Xyzz x = G1Xyzz::identity();
-    if (lane < nv)
-      for (unsigned ch = 0; ch < chunks; ch++) {
-        G1Xyzz q = ld_xyzz(classes, ((size_t)b * plan.nclasses + plan.first_class[j] + lane) * chunks + ch);
-        xyzz_add(x, q);
-      }
-    for (int d = 1; d < nv; d <<= 1) {  // inclusive suffix scan over lanes 0..nv-1
-      G1Xyzz o = shfl_down_xyzz(x, d, 32);
-      if (lane + d < nv) xyzz_add(x, o);
-    }
-    G1Xyzz y = (lane >= 1 && lane < nv) ? x : G1Xyzz::identity();
-    for (int d = nv >> 1; d > 0; d >>= 1) {
-      G1Xyzz o = shfl_down_xyzz(y, d, 32);
-      xyzz_add(y, o);
-    }
-    if (lane == 0) st_xyzz(out, (size_t)b * (plan.ndig + 1) + j, y);
-  } else if (j == 7) {
-    G1Xyzz acc = G1Xyzz::identity();
-    for (int k = lane; k < plan.n_a_classes; k += 32) {
-      G1Xyzz q = ld_xyzz(classes, ((size_t)b * plan.nclasses + plan.n_digit_classes + k) * chunks);
-      xyzz_add(acc, q);
-    }
-    acc = warp_sum(acc);
-    if (lane == 0) st_xyzz(out, (size_t)b * (plan.ndig + 1) + plan.ndig, acc);
+// n_sets sets of `chunks` consecutive points -> one sum per set; one warp per set, 4 per CTA.
+__global__ void __launch_bounds__(128) k_msm_fold(const uint4* in, unsigned n_sets, unsigned chunks, uint4* out) {
+  const unsigned set = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (set >= n_sets) return;
+  G1Xyzz acc = G1Xyzz::identity();
+  for (unsigned k = lane; k < chunks; k += 32) xyzz_add(acc, ld_xyzz(in, (size_t)set * chunks + k));
+  acc = warp_sum(acc);
+  if (lane == 0) st_xyzz(out, set, acc);
+}
+
+// sum_{k >= first} (k + 1 - first) x_k over lanes k < n of a warp (n <= 32, a power of two): inclusive suffix
+// scan, then the sum of lanes first .. n-1.  The result is in lane 0.
+PB_D G1Xyzz weighted_lane_sum(G1Xyzz x, int lane, int n, int first) {
+  for (int d = 1; d < n; d <<= 1) {
+    G1Xyzz o = shfl_down_xyzz(x, d, 32);
+    if (lane + d < n) xyzz_add(x, o);
   }
+  G1Xyzz y = (lane >= first && lane < n) ? x : G1Xyzz::identity();
+  for (int d = n >> 1; d > 0; d >>= 1) {
+    G1Xyzz o = shfl_down_xyzz(y, d, 32);
+    xyzz_add(y, o);
+  }
+  return y;
+}
+
+// out is [batch][ndig + 1]: D_0 .. D_{ndig-1}, then sum_j (j + 1) T_j.
+__global__ void __launch_bounds__(256) k_msm_final(const uint4* lists, DigitPlan plan, unsigned chunks, uint4* out) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const unsigned b = blockIdx.x;
+  if (w >= plan.ndig && w != 7) return;
+  const bool digit = w < plan.ndig;
+  const int n = digit ? 1 << plan.bits[w] : plan.n_columns;
+  const int first_list = digit ? plan.first_class[w] : plan.n_digit_classes;
+  G1Xyzz x = G1Xyzz::identity();
+  if (lane < n)
+    for (unsigned ch = 0; ch < chunks; ch++) xyzz_add(x, ld_xyzz(lists, ((size_t)b * plan.nlists + first_list + lane) * chunks + ch));
+  // D_j = sum_v v C_{j,v} (lane 0 holds class v = 0, weight 0); the columns carry weights 1 .. g
+  const G1Xyzz y = weighted_lane_sum(x, lane, n, digit ? 1 : 0);
+  if (lane == 0) st_xyzz(out, (size_t)b * (plan.ndig + 1) + (digit ? w : plan.ndig), y);
 }
 
 __global__ void k_selftest_fr_mul(const uint4* a, const uint4* b, uint4* o, size_t n) {
@@ -1136,6 +1165,9 @@ static void xyzz_dev_to_host(const uint32_t* w, pbh::HXyzz* o) {
 // Set by a caller that keeps several MSMs in flight on other streams (prover.cu): dense MSMs then use one lane
 // per bucket (no merge additions).  Thread-local: an MSM is enqueued by the thread that owns its stream.
 thread_local int t_msm_throughput_hint = 0;
+// Set by the same caller for an MSM that keeps its latency-oriented bucket split (the sparse wire MSM) while other
+// proofs are in flight: only its over-long buckets switch to the wide chunks.
+thread_local int t_msm_wide_heavy_chunks = 0;
 
 // What the host needs to finish an MSM whose kernels have been enqueued: the digit plan of the bucket
 // reduction.  It depends on the window width of the key only, never on the number of scalars, so the
@@ -1189,8 +1221,8 @@ static int msm_plan_c(int c, uint32_t batch, MsmTail* tail, unsigned* n_groups_o
     cls += 1 << bits;
   }
   plan.n_digit_classes = cls;
-  plan.n_a_classes = (int)((n_groups + 255) / 256);
-  plan.nclasses = plan.n_digit_classes + plan.n_a_classes;
+  plan.n_columns = g;
+  plan.nlists = plan.n_digit_classes + plan.n_columns;
   tail->log_g = log_g;
   tail->c = c;
   tail->batch = batch;
@@ -1200,6 +1232,13 @@ static int msm_plan_c(int c, uint32_t batch, MsmTail* tail, unsigned* n_groups_o
 }
 static int msm_plan(const pb200_srs* srs, uint32_t batch, MsmTail* tail, unsigned* n_groups_out, int* g_out) {
   return msm_plan_c(srs->c, batch, tail, n_groups_out, g_out);
+}
+
+// kListChunk-member chunks of the longest list of k_msm_lists (n_parts partials per column)
+static unsigned reduction_chunks(const DigitPlan& plan, unsigned n_groups, unsigned n_parts) {
+  unsigned chunks = (n_parts + kListChunk - 1) / kListChunk;
+  for (int j = 0; j < plan.ndig; j++) chunks = std::max(chunks, ((n_groups >> plan.bits[j]) + kListChunk - 1) / kListChunk);
+  return std::max(chunks, 1u);
 }
 
 // Enqueues every kernel of `batch` MSMs over the points [first, first + n) of the key on `st`.  The
@@ -1238,7 +1277,7 @@ static int msm_enqueue(const pb200_srs* srs, size_t first, const uint64_t* d_sca
   if (const char* env = getenv("PB200_MSM_LOG_SPLIT")) log_split = atoi(env);
 
   unsigned *counts = nullptr, *offsets = nullptr, *order = nullptr, *ebkt = nullptr, *epos = nullptr, *sorted = nullptr;
-  uint4 *sums = nullptr, *classes = nullptr, *S = nullptr, *A = nullptr;
+  uint4 *sums = nullptr, *lists = nullptr, *S = nullptr, *P = nullptr;
   PB_ALLOC(scope, counts, (size_t)batch * nb * 4);
   PB_ALLOC(scope, offsets, (size_t)batch * (nb + 1) * 4);
   PB_ALLOC(scope, order, (size_t)batch * nb * 4);
@@ -1251,22 +1290,23 @@ static int msm_enqueue(const pb200_srs* srs, size_t first, const uint64_t* d_sca
   PB_ALLOC(scope, epos, (size_t)batch * cap * 4);
   PB_ALLOC(scope, sorted, (size_t)batch * cap * 4);
   PB_ALLOC(scope, sums, (size_t)batch * nb * 192);
-  unsigned chunks = 1;
-  for (int j = 0; j < plan.ndig; j++) chunks = std::max<unsigned>(chunks, (unsigned)(((n_groups >> plan.bits[j]) + kClassChunk - 1) / kClassChunk));
-  PB_ALLOC(scope, classes, (size_t)batch * plan.nclasses * chunks * 192);
+  const unsigned col_run = std::min(kColRun, n_groups), n_parts = n_groups / col_run;
+  const unsigned chunks = reduction_chunks(plan, n_groups, n_parts);
+  PB_ALLOC(scope, lists, (size_t)batch * plan.nlists * chunks * 192);
   PB_ALLOC(scope, S, (size_t)batch * n_groups * 192);
-  PB_ALLOC(scope, A, (size_t)batch * n_groups * 192);
+  PB_ALLOC(scope, P, (size_t)batch * g * n_parts * 192);
   PB_CUDA(cudaMemsetAsync(counts, 0, (size_t)batch * nb * 4, st));
 
   PB_LAUNCH(k_msm_digits, dim3(div_up(n, 128), batch), 128, 0, st, (const uint4*)d_scalars, n, stride, c, W, nb,
             counts, ebkt, epos);
   int size_shift = 0;  // size unit: average bucket ~ 64 units
   while (((cap / nb) >> size_shift) > 64) size_shift++;
-  // chunk sums of the heavy buckets: at most cap / kHeavyChunk full chunks plus one ragged chunk per heavy bucket
+  // chunk sums of the heavy buckets: at most cap / heavy_chunk full chunks plus one ragged chunk per heavy bucket
+  const unsigned heavy_chunk = (t_msm_throughput_hint || t_msm_wide_heavy_chunks) ? kHeavyChunkWide : kHeavyChunk;
   const size_t part_cap = cap / kHeavyChunk + std::min<size_t>(nb, cap / kHeavyMin) + 2;
   uint4* partials = nullptr;
   PB_ALLOC(scope, partials, (size_t)batch * part_cap * 192);
-  PB_LAUNCH(k_msm_scan, batch, 1024, 0, st, counts, offsets, order, n_heavy, heavy_pre, max_len, nb, size_shift);
+  PB_LAUNCH(k_msm_scan, batch, 1024, 0, st, counts, offsets, order, n_heavy, heavy_pre, max_len, nb, size_shift, heavy_chunk);
   PB_LAUNCH(k_msm_scatter, dim3(div_up(n, 256), W, batch), 256, 0, st, ebkt, epos, offsets, n, W, nb,
             srs->n_points, first, sorted);
   if (prof_ev) PB_CUDA(cudaEventRecord(prof_ev[0], st));
@@ -1317,7 +1357,7 @@ static int msm_enqueue(const pb200_srs* srs, size_t first, const uint64_t* d_sca
     }
     if (prof_ev) PB_CUDA(cudaEventRecord(prof_ev[1], st));
     if (d_totals) *d_totals = offsets + nb;
-    PB_LAUNCH(k_msm_groups<true>, dim3(div_up(n_groups, 64), batch), 64, 0, st, (const uint4*)sums, nb, g, S, A);
+    PB_LAUNCH(k_msm_rows_cols<true>, dim3(div_up(n_groups + g * n_parts, 64), batch), 64, 0, st, (const uint4*)sums, nb, (unsigned)g, col_run, S, P);
   } else {
   {
     // CTA shape: 64 threads x 4 CTAs/SM and 128 x 2 hold the same 8 warps per SM (register-limited);
@@ -1336,14 +1376,20 @@ static int msm_enqueue(const pb200_srs* srs, size_t first, const uint64_t* d_sca
     }
   }
   if (d_totals) *d_totals = offsets + nb;  // offsets[b][nb] = the entries of batch b (stride nb + 1)
-  PB_LAUNCH(k_msm_heavy_chunks, dim3(4 * num_sms(), batch), 128, 0, st, srs->table, sorted, offsets, order, n_heavy, heavy_pre, nb, cap, part_cap, partials);
+  PB_LAUNCH(k_msm_heavy_chunks, dim3(4 * num_sms(), batch), 128, 0, st, srs->table, sorted, offsets, order, n_heavy, heavy_pre, nb, heavy_chunk, cap,
+            part_cap, partials);
   PB_LAUNCH(k_msm_heavy_combine, dim3(64, batch), 128, 0, st, (const uint4*)partials, order, n_heavy, heavy_pre, nb, part_cap, sums);
   if (prof_ev) PB_CUDA(cudaEventRecord(prof_ev[1], st));  // the bucket-accumulation phase: every entry has been added once
-    PB_LAUNCH(k_msm_groups<false>, dim3(div_up(n_groups, 64), batch), 64, 0, st, (const uint4*)sums, nb, g, S, A);
+    PB_LAUNCH(k_msm_rows_cols<false>, dim3(div_up(n_groups + g * n_parts, 64), batch), 64, 0, st, (const uint4*)sums, nb, (unsigned)g, col_run, S, P);
   }
-  PB_LAUNCH(k_msm_group_classes, dim3(div_up(plan.nclasses, 4), batch, chunks), 128, 0, st, (const uint4*)S, (const uint4*)A,
-            n_groups, plan, chunks, classes);
-  PB_LAUNCH(k_msm_final, batch, 256, 0, st, (const uint4*)classes, plan, chunks, result);
+  PB_LAUNCH(k_msm_lists, dim3(div_up(plan.nlists, 4), batch, chunks), 128, 0, st, (const uint4*)S, (const uint4*)P, n_groups, n_parts, plan,
+            chunks, lists);
+  if (chunks > kFinalChunks) {  // S is dead: it takes the folded list sums
+    PB_LAUNCH(k_msm_fold, div_up((size_t)batch * plan.nlists, 4), 128, 0, st, (const uint4*)lists, batch * (unsigned)plan.nlists, chunks, S);
+    PB_LAUNCH(k_msm_final, batch, 256, 0, st, (const uint4*)S, plan, 1u, result);
+  } else {
+    PB_LAUNCH(k_msm_final, batch, 256, 0, st, (const uint4*)lists, plan, chunks, result);
+  }
   PB_CUDA(cudaGetLastError());
   return 0;
 }
@@ -1541,7 +1587,11 @@ int msm_allgather(const pb200_srs* srs, const uint64_t* scalars, bool scalars_on
 // Upper bound of the arena bytes one msm_run(n, batch) call takes (same list as the PB_ALLOCs above).
 size_t msm_workspace_bytes(const pb200_srs* srs, size_t n, uint32_t batch) {
   const size_t nb = (size_t)1 << (srs->c - 1), cap = n * (size_t)srs->W;
-  const size_t n_groups = std::max<size_t>(1, nb / kGroup);
+  MsmTail tail;
+  unsigned n_groups = 0;
+  int g = 0;
+  if (msm_plan(srs, batch, &tail, &n_groups, &g) != 0) return 0;
+  const unsigned n_parts = n_groups / std::min(kColRun, n_groups);
   size_t b = 0;
   b += 4 * ((size_t)batch * (nb + 1) * 4 + 256);      // counts, offsets, order, heavy_pre
   {
@@ -1552,8 +1602,9 @@ size_t msm_workspace_bytes(const pb200_srs* srs, size_t n, uint32_t batch) {
   b += (size_t)batch * 4 + 256;                        // n_heavy
   b += 3 * ((size_t)batch * cap * 4 + 256);            // ebkt, epos, sorted
   b += (size_t)batch * nb * 192 + 256;                 // sums
-  b += 2 * ((size_t)batch * n_groups * 192 + 256);     // S, A
-  b += (size_t)batch * (8 * 16 + n_groups / 256 + 2) * (n_groups / (16 * kClassChunk) + 2) * 192 + 256;  // classes x chunks
+  b += (size_t)batch * n_groups * 192 + 256;           // S
+  b += (size_t)batch * g * n_parts * 192 + 256;        // P
+  b += (size_t)batch * tail.plan.nlists * reduction_chunks(tail.plan, n_groups, n_parts) * 192 + 256;  // lists x chunks
   b += (size_t)batch * 9 * 192 + 256;                  // result
   if (msm_affine_enabled()) {  // batched-affine rounds: two point buffers, running products, pair descriptors
     b += (size_t)batch * ((cap / 2 + nb + 2) + (cap / 4 + nb + 2)) * 96 + 512;

@@ -41,6 +41,7 @@ const uint4* srs_points(const pb200_srs* s);
 int srs_from_device(const uint4* d_points, size_t n_points, pb200_srs** out, int window_bits);
 int msm_window_for(size_t n_points);
 extern thread_local int t_msm_throughput_hint;
+extern thread_local int t_msm_wide_heavy_chunks;
 // pb200_throughput_mode(1): treat every proof as one of many in flight (a measurement aid: bench.py times the
 // dominant kernel with single proofs but wants the launch shape of its timed region)
 static std::atomic<int> g_force_throughput{0};
@@ -991,6 +992,7 @@ int prove_dev(const pb200_prover* P, const uint64_t* d_wit, const uint64_t* pi_i
     ~InFlight() {
       P->active.fetch_sub(1, std::memory_order_relaxed);
       t_msm_throughput_hint = 0;
+      t_msm_wide_heavy_chunks = 0;
     }
   } in_flight(P);
   static const int hint_at = [] {  // PB200_THROUGHPUT_AT=<k>: proofs in flight from which the hint is given (0 = never)
@@ -1094,7 +1096,9 @@ int prove_dev(const pb200_prover* P, const uint64_t* d_wit, const uint64_t* pi_i
       for (int i = 0; i < 2; i++) ba.b[p][i] = to_dev(BL[2 * p + i]);
     PB_LAUNCH(k_lagrange_tail, 1, 32, 0, st, sc, stride, n, ba);
     t_msm_throughput_hint = 0;  // sparse scalars: long buckets want their lanes
+    t_msm_wide_heavy_chunks = (hint_at > 0 && (g_force_throughput.load(std::memory_order_relaxed) || P->active.load(std::memory_order_relaxed) >= hint_at)) ? 1 : 0;
     PB_TRY(msm_run(P->srs_lag, 0, (const uint64_t*)sc, n + 4, 4, stride, aff, st, ar));
+    t_msm_wide_heavy_chunks = 0;
   } else {
     t_msm_throughput_hint = (hint_at > 0 && (g_force_throughput.load(std::memory_order_relaxed) || P->active.load(std::memory_order_relaxed) >= hint_at)) ? 1 : 0;
     PB_TRY(msm_run(P->srs, 0, (const uint64_t*)wp, n + 2, 4, stride, aff, st, ar));
