@@ -8,12 +8,12 @@ OBJ=${PB200_OBJ:-build/obj}
 mkdir -p $OBJ
 NVFLAGS="-std=c++17 -O3 -lineinfo -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC -Xcompiler -O2 $*"
 pids=()
-for f in capi ntt msm prover ecntt; do
+for f in capi ntt msm prover ecntt verify; do
   nvcc $NVFLAGS -c -o $OBJ/$f.o $SRC/$f.cu &
   pids+=($!)
 done
 g++ -std=c++17 -O2 -fPIC -c -o $OBJ/host_field.o $SRC/host_field.cpp
 g++ -std=c++17 -O2 -fPIC -c -o $OBJ/composer.o $SRC/composer.cpp
 for p in "${pids[@]}"; do wait $p; done
-nvcc -shared -o "$OUT" $OBJ/capi.o $OBJ/ntt.o $OBJ/msm.o $OBJ/prover.o $OBJ/ecntt.o $OBJ/host_field.o $OBJ/composer.o
+nvcc -shared -o "$OUT" $OBJ/capi.o $OBJ/ntt.o $OBJ/msm.o $OBJ/prover.o $OBJ/ecntt.o $OBJ/verify.o $OBJ/host_field.o $OBJ/composer.o
 echo "built $OUT"

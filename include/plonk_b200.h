@@ -47,12 +47,14 @@ typedef enum {
   PB200_ERR_UNSATISFIED = -5,     /* Error::CircuitUnsatisfied (quotient_poly.rs:132-134) */
   PB200_ERR_NOT_READY = -6,
   /* -7 .. -9: circuit front end, plonk_b200_composer.h */
-  PB200_ERR_POINT_MALFORMED = -10 /* dusk_bytes::Error::InvalidData / Error::PointMalformed: a G1 encoding that is
+  PB200_ERR_POINT_MALFORMED = -10,/* dusk_bytes::Error::InvalidData / Error::PointMalformed: a G1 encoding that is
                                      not canonical, not on the curve or not in the prime-order subgroup */
+  PB200_ERR_VERIFY = -11          /* Error::ProofVerificationError: the proof does not satisfy the verifier */
 } pb200_status;
 
 typedef struct pb200_srs pb200_srs_t;
 typedef struct pb200_prover pb200_prover_t;
+typedef struct pb200_verifier pb200_verifier_t;
 
 /* ---- process / device ------------------------------------------------------------------- */
 /* Selects the device for this process.  Idempotent for the same device; ONE device per process: the
@@ -211,6 +213,38 @@ int pb200_prove(const pb200_prover_t* prover, const uint64_t* witnesses, size_t 
 int pb200_prove_dev(const pb200_prover_t* prover, const uint64_t* d_witnesses, size_t n_witnesses,
                     const uint64_t* pi_idx, const uint64_t* pi_vals, size_t n_pi,
                     const uint64_t* blinders, uint8_t* out_proof, void* stream);
+
+/* ---- verifier (Verifier::verify, PlonkVersion::V3; src/compiler/verifier.rs) ---------------------------------- */
+/* Compiler::compile's Verifier half: the label, the circuit's constraint count, the 15 verifier-key commitments in
+ * pb200_prover_commitments order, OpeningKey::to_bytes (PB200_OPENING_KEY_BYTES: g compressed, then h and [x]h as
+ * 96-byte compressed G2 points - zcash encoding, x.c1 then x.c0 big-endian) and the public-input positions.
+ * The commitments and g are decoded with the on-curve and subgroup checks; an identity, off-curve or non-subgroup
+ * opening-key point is PB200_ERR_POINT_MALFORMED (OpeningKey::try_new, key.rs:620-648).  The lines of h and [x]h
+ * (G2Prepared) are computed on the device once, here. */
+int pb200_verifier_new(const uint8_t* label, size_t label_len, size_t n_constraints, const uint8_t* vk_comms_15x48,
+                       const uint8_t* opening_key, const uint64_t* pi_idx, size_t n_pi, pb200_verifier_t** out);
+/* Verifier::try_from_bytes / Verifier::to_bytes (verifier.rs:62-202).  Layout: six big-endian u64 (label length,
+ * verifier-key length = 968, opening-key length = 240, public-input count, size, constraints), the label,
+ * VerifierKey::to_bytes (widget.rs:84-135: n - the constraint count, compiler.rs:278-279 - as a little-endian u64, then the commitments q_m, q_l, q_r, q_o, q_f,
+ * q_c, q_arith, q_logic, q_range, q_fixed_group_add, q_variable_group_add, s_sigma_1..4 compressed, then zeros up to
+ * 20 x 48 + 8 bytes), OpeningKey::to_bytes and one big-endian u64 per public-input position.  from_bytes: lengths
+ * that do not fit the bytes or overflow -> PB200_ERR_INVALID_ARG (NotEnoughBytes); a malformed point ->
+ * PB200_ERR_POINT_MALFORMED; a domain (the next power of two of VerifierKey::n) of 2^32 or more -> PB200_ERR_INVALID_DOMAIN.  to_bytes writes *len bytes to
+ * `out` (out = NULL: only *len). */
+int pb200_verifier_from_bytes(const uint8_t* bytes, size_t len, pb200_verifier_t** out);
+int pb200_verifier_to_bytes(const pb200_verifier_t* verifier, uint8_t* out, size_t cap, size_t* len);
+void pb200_verifier_free(pb200_verifier_t* verifier);
+/* Verifier::verify for n_proofs proofs of 1008 bytes (Proof::to_bytes), each with n_pi public inputs (pi_vals:
+ * n_proofs x n_pi Fr, Montgomery form).  status[i] is the proof's verdict: PB200_OK, PB200_ERR_VERIFY (the
+ * pairing check fails, or z lies in the domain) or PB200_ERR_POINT_MALFORMED (Proof::from_bytes would fail: a
+ * commitment that is not canonical, not on the curve or not torsion free, or a non-canonical evaluation).  A verdict
+ * does not depend on the batch.  The call itself fails with PB200_ERR_INVALID_ARG when n_pi differs from the
+ * verifier's public-input count (InconsistentPublicInputsLen). */
+int pb200_verify(const pb200_verifier_t* verifier, const uint8_t* proofs, size_t n_proofs, const uint64_t* pi_vals,
+                 size_t n_pi, int32_t* status);
+/* Tests only: the device pairing e(P_k, Q_k) for n G1 points (96-byte raw layout) and n compressed G2 points, as
+ * Fp12 values of 576 bytes (c0.c0.c0, c0.c0.c1, c0.c1.c0, ..., c1.c2.c1; each Fp 6 x u64 Montgomery limbs). */
+int pb200_selftest_pairing(const uint64_t* g1_raw, const uint8_t* g2_compressed, size_t n, uint64_t* out_fp12);
 
 /* ---- measurement helpers ----------------------------------------------------------------- */
 /* In-library CUDA-event timing of the MSM bucket-accumulation phase (k_msm_accumulate, the dominant

@@ -7,6 +7,7 @@
 //   plonk_b200::CommitKey          src/commitment_scheme/kzg10/key.rs:36-41, 362-388   commit, max_degree
 //   plonk_b200::Commitment         src/commitment_scheme/kzg10/commitment.rs:77-106    to_bytes (48 B)
 //   plonk_b200::Prover             src/compiler/prover.rs:53-115, 352-362              prove
+//   plonk_b200::Verifier           src/compiler/verifier.rs:32-262                     verify, to_bytes, try_from_bytes
 //   plonk_b200::Composer           src/composer.rs:72-495 + src/composer/{bits,range,logic,truncate,select,
 //                                  point,fixed_base}.rs (host-side circuit front end, plonk_b200_composer.h)
 //   plonk_b200::Error              src/error.rs:21-120 (the variants this path can produce)
@@ -32,7 +33,9 @@ using BlsScalar = std::array<uint64_t, 4>;
 struct Error : std::runtime_error {
   enum Kind {
     InvalidEvalDomainSize, PolynomialDegreeTooLarge, CircuitUnsatisfied, InvalidArgument, BackendFailure,
-    JubJubPointNotTorsionFree, JubJubGeneratorNotPrimeOrder, JubJubScalarMalformed
+    JubJubPointNotTorsionFree, JubJubGeneratorNotPrimeOrder, JubJubScalarMalformed,
+    ProofVerificationError,  // Error::ProofVerificationError
+    PointMalformed           // Error::BytesError(dusk_bytes::Error::InvalidData) of the verifier's decoders
   };
   Kind kind;
   Error(Kind k, const std::string& what) : std::runtime_error(what), kind(k) {}
@@ -351,6 +354,69 @@ class Prover {
   Prover() : n_witnesses_(0) {}
   pb200_prover_t* h_ = nullptr;
   size_t n_witnesses_;
+};
+
+// Verifier (PlonkVersion::V3).  Errors as the reference: verify() throws ProofVerificationError for a proof that
+// fails the check, PointMalformed for one Proof::from_bytes refuses, InvalidArgument for a public-input count that
+// is not the verifier's (InconsistentPublicInputsLen); the constructors throw PointMalformed for a degenerate opening
+// key, InvalidArgument for truncated or overflowing bytes (NotEnoughBytes), InvalidEvalDomainSize for a domain of
+// 2^32 or more.
+class Verifier {
+ public:
+  static constexpr size_t PROOF_SIZE = 1008;                      // Proof::SIZE
+  static constexpr size_t OPENING_KEY_SIZE = PB200_OPENING_KEY_BYTES;  // OpeningKey::SIZE
+  // Compiler::compile's Verifier half: the 15 commitments in Prover::commitments order (pb200_prover_commitments)
+  Verifier(const std::string& label, size_t n_constraints, const std::array<uint8_t, 15 * 48>& commitments,
+           const std::array<uint8_t, OPENING_KEY_SIZE>& opening_key, const std::vector<uint64_t>& pi_idx) {
+    check_verifier(pb200_verifier_new((const uint8_t*)label.data(), label.size(), n_constraints, commitments.data(), opening_key.data(),
+                                      pi_idx.empty() ? nullptr : pi_idx.data(), pi_idx.size(), &h_));
+  }
+  static std::unique_ptr<Verifier> try_from_bytes(const uint8_t* bytes, size_t len) {
+    std::unique_ptr<Verifier> v(new Verifier());
+    check_verifier(pb200_verifier_from_bytes(bytes, len, &v->h_));
+    return v;
+  }
+  ~Verifier() { pb200_verifier_free(h_); }
+  Verifier(const Verifier&) = delete;
+  Verifier& operator=(const Verifier&) = delete;
+  std::vector<uint8_t> to_bytes() const {
+    size_t n = 0;
+    check(pb200_verifier_to_bytes(h_, nullptr, 0, &n));
+    std::vector<uint8_t> out(n);
+    check(pb200_verifier_to_bytes(h_, out.data(), out.size(), &n));
+    return out;
+  }
+  // Verifier::verify
+  void verify(const std::array<uint8_t, PROOF_SIZE>& proof, const std::vector<BlsScalar>& public_inputs) const {
+    const std::vector<int32_t> st = verify_batch({proof}, {public_inputs});
+    if (st[0] == PB200_ERR_POINT_MALFORMED) throw Error(Error::PointMalformed, "InvalidData: malformed proof");
+    check_verifier(st[0]);
+  }
+  // One status per proof (PB200_OK, PB200_ERR_VERIFY or PB200_ERR_POINT_MALFORMED); every proof must come with the
+  // same number of public inputs.
+  std::vector<int32_t> verify_batch(const std::vector<std::array<uint8_t, PROOF_SIZE>>& proofs,
+                                    const std::vector<std::vector<BlsScalar>>& public_inputs) const {
+    if (proofs.size() != public_inputs.size()) throw Error(Error::InvalidArgument, "one public-input vector per proof");
+    const size_t n_pi = public_inputs.empty() ? 0 : public_inputs[0].size();
+    std::vector<BlsScalar> pi;
+    for (const auto& v : public_inputs) {
+      if (v.size() != n_pi) throw Error(Error::InvalidArgument, "every proof needs the same number of public inputs");
+      pi.insert(pi.end(), v.begin(), v.end());
+    }
+    std::vector<int32_t> st(proofs.size());
+    check_verifier(pb200_verify(h_, proofs.empty() ? nullptr : proofs[0].data(), proofs.size(), pi.empty() ? nullptr : pi[0].data(),
+                                n_pi, st.data()));
+    return st;
+  }
+
+ private:
+  Verifier() = default;
+  static void check_verifier(int rc) {
+    if (rc == PB200_ERR_VERIFY) throw Error(Error::ProofVerificationError, "ProofVerificationError");
+    if (rc == PB200_ERR_POINT_MALFORMED) throw Error(Error::PointMalformed, std::string("InvalidData: ") + pb200_last_error());
+    check(rc);
+  }
+  pb200_verifier_t* h_ = nullptr;
 };
 
 }  // namespace plonk_b200

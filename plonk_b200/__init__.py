@@ -10,3 +10,4 @@ from ._lib import Pb200Error, lib  # noqa: F401
 from .domain import EvaluationDomain  # noqa: F401
 from .kzg import CommitKey, Commitment, PolynomialDegreeTooLarge  # noqa: F401
 from .prover import CircuitUnsatisfied, Prover  # noqa: F401
+from .verifier import PointMalformed, ProofVerificationError, Verifier  # noqa: F401

@@ -17,6 +17,7 @@ PB200_ERR_DEGREE_TOO_LARGE = -3
 PB200_ERR_INVALID_ARG = -4
 PB200_ERR_UNSATISFIED = -5
 PB200_ERR_POINT_MALFORMED = -10
+PB200_ERR_VERIFY = -11
 
 _lib = None
 
@@ -29,7 +30,8 @@ EXPORTS = [
     "pb200_g1_compress", "pb200_g1_decompress", "pb200_raw_commit_key_points", "pb200_commit_key_from_raw_var_bytes", "pb200_g1_add_affine", "pb200_srs_setup_from_secret", "pb200_g1_lagrange_key",
     "pb200_profile_enable", "pb200_throughput_mode", "pb200_profile_read", "pb200_profile_read_sparse",
     "pb200_prover_new", "pb200_prover_from_bytes", "pb200_prover_free", "pb200_prover_commitments", "pb200_prove", "pb200_prove_dev",
-    "pb200_imad_peak", "pb200_fp_product_peak", "pb200_selftest_fr_mul", "pb200_selftest_fp_mul", "pb200_selftest_fp_ops",
+    "pb200_verifier_new", "pb200_verifier_from_bytes", "pb200_verifier_to_bytes", "pb200_verifier_free", "pb200_verify",
+    "pb200_imad_peak", "pb200_fp_product_peak", "pb200_selftest_pairing", "pb200_selftest_fr_mul", "pb200_selftest_fp_mul", "pb200_selftest_fp_ops",
 ]
 
 
@@ -109,6 +111,13 @@ def lib() -> ctypes.CDLL:
         L.pb200_fp_product_peak.argtypes = [c.POINTER(c.c_double)]
         L.pb200_selftest_fr_mul.argtypes = [c.c_void_p, c.c_void_p, c.c_void_p, c.c_size_t]
         L.pb200_selftest_fp_mul.argtypes = [c.c_void_p, c.c_void_p, c.c_void_p, c.c_size_t]
+        L.pb200_verifier_new.argtypes = [c.c_void_p, c.c_size_t, c.c_size_t, c.c_void_p, c.c_void_p, c.c_void_p, c.c_size_t, c.POINTER(c.c_void_p)]
+        L.pb200_verifier_from_bytes.argtypes = [c.c_void_p, c.c_size_t, c.POINTER(c.c_void_p)]
+        L.pb200_verifier_to_bytes.argtypes = [c.c_void_p, c.c_void_p, c.c_size_t, c.POINTER(c.c_size_t)]
+        L.pb200_verifier_free.argtypes = [c.c_void_p]
+        L.pb200_verifier_free.restype = None
+        L.pb200_verify.argtypes = [c.c_void_p, c.c_void_p, c.c_size_t, c.c_void_p, c.c_size_t, c.c_void_p]
+        L.pb200_selftest_pairing.argtypes = [c.c_void_p, c.c_void_p, c.c_size_t, c.c_void_p]
         _bind_composer(L)
         _lib = L
     return _lib

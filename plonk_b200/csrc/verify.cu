@@ -1,0 +1,610 @@
+// Verifier (reference src/compiler/verifier.rs) for PlonkVersion::V3 proofs: Verifier::verify for a batch of proofs
+// per call, one verdict per proof.
+//
+// The host parses, replays the transcript and computes the O(#public inputs) scalars of Proof::verify
+// (src/proof_system/proof.rs:218-516).  The device decodes the commitments (k_g1_decompress), forms the two G1
+// points of the final pairing check with one warp per proof (k_verify_msm), and runs the multi-Miller loop, the
+// final exponentiation and the comparison with 1 with one thread per proof (k_verify_pairing).
+#include <algorithm>
+#include <mutex>
+#include <thread>
+#include <vector>
+
+#include "common.cuh"
+#include "g1.cuh"
+#include "host_field.h"
+#include "pairing.cuh"
+#include "transcript.h"
+
+struct pb200_verifier {
+  std::vector<uint8_t> label;
+  uint64_t vk_n = 0;                          // VerifierKey::n: the constraint count for a compiled circuit
+  uint64_t n = 0, size = 0, constraints = 0;  // the domain size (EvaluationDomain::new(vk_n)), Verifier::size, Verifier::constraints
+  uint8_t vk_comm[15][48];                     // pb200_prover_commitments order
+  uint8_t opening_key[PB200_OPENING_KEY_BYTES];
+  std::vector<uint64_t> pi_idx;
+  std::vector<pbh::HFr> pi_roots;  // group_gen_inv^index
+  pbh::HFr group_gen, size_fr, size_inv;
+  pbh::Transcript base;
+  uint4* d_points = nullptr;        // the 15 key commitments then opening_key.g, 96-byte raw affine
+  pb::LineCoeffs* d_lines = nullptr;  // prepared [x]H then H, PB_G2_LINES each
+  pb200_verifier() : base(nullptr, 0) {}
+};
+
+namespace pb {
+void g1_decompress_dev(const uint8_t* d_in, size_t n, uint4* d_out, unsigned* d_bad, cudaStream_t st);
+int g1_decompress(const uint8_t* in, size_t n, int check_subgroup, uint8_t* out_raw);
+
+namespace {
+using pbh::HFr;
+
+PB_D G1Affine ld_aff(const uint4* q) {
+  G1Affine p;
+  const uint32_t* w = (const uint32_t*)q;
+#pragma unroll
+  for (int k = 0; k < 12; k++) {
+    p.x.v[k] = w[k];
+    p.y.v[k] = w[12 + k];
+  }
+  return p;
+}
+PB_D void st_aff(uint4* q, const G1Affine& p) {
+  uint32_t* w = (uint32_t*)q;
+#pragma unroll
+  for (int k = 0; k < 12; k++) {
+    w[k] = p.x.v[k];
+    w[12 + k] = p.y.v[k];
+  }
+}
+PB_D G1Xyzz shfl_down_xyzz(const G1Xyzz& a, int d) {
+  G1Xyzz r;
+#pragma unroll
+  for (int k = 0; k < 12; k++) {
+    r.x.v[k] = __shfl_down_sync(0xffffffffu, a.x.v[k], d);
+    r.y.v[k] = __shfl_down_sync(0xffffffffu, a.y.v[k], d);
+    r.zz.v[k] = __shfl_down_sync(0xffffffffu, a.zz.v[k], d);
+    r.zzz.v[k] = __shfl_down_sync(0xffffffffu, a.zzz.v[k], d);
+  }
+  return r;
+}
+PB_D G1Affine to_affine(const G1Xyzz& p) {
+  if (p.is_inf()) return {Fp::zero(), Fp::zero()};
+  const Fp i = fp_inv_bingcd(p.zz * p.zzz);
+  return {p.x * (i * p.zzz), p.y * (i * p.zz)};
+}
+
+// Lane k of a warp multiplies term k of right_projective (proof.rs:300-455): the source of its point is a key
+// point (0..15: the 15 commitments in pb200_prover_commitments order, then opening_key.g) or a proof commitment
+// (16 + its index in Proof::to_bytes order); -1 = no term.  Lane 31 computes u [W_zw] + [W_z] for left_projective.
+enum { P_A = 16, P_B, P_C, P_D, P_Z, P_TLOW, P_TMID, P_THIGH, P_TFOURTH, P_WZ, P_WZW };
+__constant__ int c_term_point[32] = {0,  1,  2,  3,       4,      5,      7,       8,         9,    10, P_Z,   14, P_TLOW, P_TMID, P_THIGH, P_TFOURTH,
+                                     P_A, P_B, P_C, P_D, 11, 12, 13, 6, 5, 1, 2, 15, P_WZ, P_WZW, -1, P_WZW};
+#define PB_VERIFY_TERMS 32
+
+// One warp per proof.  scalars: [proof][32] canonical little-endian Fr; proof_comm: [proof][11] compressed
+// commitments; pts: their decoded points.  status: PB200_OK on entry or the host's verdict; a commitment that
+// decoded to zeros without being the identity's encoding is malformed.  out: [proof] -(W_z + u W_zw), right.
+__global__ void __launch_bounds__(128) k_verify_msm(const uint4* key_pts, const uint4* pts, const uint8_t* proof_comm,
+                                                    const uint4* scalars, size_t n, int* status, uint4* out) {
+  const size_t i = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (i >= n) return;  // whole warps
+  bool bad = false;
+  if (lane < 11) {
+    const uint4* q = pts + 6 * (i * 11 + lane);
+    const G1Affine p = ld_aff(q);
+    if (p.is_inf()) {
+      const uint8_t* e = proof_comm + 48 * (i * 11 + lane);
+      uint32_t acc = e[0] ^ 0xc0u;
+      for (int k = 1; k < 48; k++) acc |= e[k];
+      bad = acc != 0;
+    }
+  }
+  if (__any_sync(0xffffffffu, bad)) {
+    if (lane == 0) status[i] = PB200_ERR_POINT_MALFORMED;
+    return;
+  }
+  if (status[i] != PB200_OK) return;
+  G1Xyzz acc = G1Xyzz::identity();
+  const int src = c_term_point[lane];
+  if (src >= 0) {
+    const G1Affine p = src < 16 ? ld_aff(key_pts + 6 * src) : ld_aff(pts + 6 * (i * 11 + (src - 16)));
+    if (!p.is_inf()) {
+      const uint4* sp = scalars + 2 * (i * PB_VERIFY_TERMS + lane);
+      const uint4 lo = sp[0], hi = sp[1];
+      const uint32_t s[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
+#pragma unroll 1
+      for (int w = 7; w >= 0; w--) {
+#pragma unroll 1
+        for (int b = 31; b >= 0; b--) {
+          acc = xyzz_dbl(acc);
+          if ((s[w] >> b) & 1u) xyzz_madd(acc, p.x, p.y);
+        }
+      }
+    }
+  }
+  G1Xyzz left = G1Xyzz::identity();
+  if (lane == 31) {
+    const G1Affine wz = ld_aff(pts + 6 * (i * 11 + (P_WZ - 16)));
+    left = acc;
+    if (!wz.is_inf()) xyzz_madd(left, wz.x, wz.y);
+    left = left.neg();
+    acc = G1Xyzz::identity();
+  }
+#pragma unroll 1
+  for (int d = 16; d >= 1; d >>= 1) {
+    const G1Xyzz o = shfl_down_xyzz(acc, d);
+    xyzz_add(acc, o);
+  }
+  if (lane == 0) st_aff(out + 12 * i + 6, to_affine(acc));
+  if (lane == 31) st_aff(out + 12 * i, to_affine(left));
+}
+
+// One thread per proof: e(-(W_z + u W_zw), [x]H) e(right, H) == 1 (proof.rs:498-513).
+__global__ void __launch_bounds__(64) k_verify_pairing(const uint4* g1, const LineCoeffs* lines, size_t n, int* status) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n || status[i] != PB200_OK) return;
+  G1Affine p[2] = {ld_aff(g1 + 12 * i), ld_aff(g1 + 12 * i + 6)};
+  const LineCoeffs* l[2] = {lines, lines + PB_G2_LINES};
+  const Fp12 f = final_exponentiation(miller_loop2(p, l));
+  status[i] = f.is_one() ? PB200_OK : PB200_ERR_VERIFY;
+}
+
+// Decodes `count` G2 points (96-byte encodings) and prepares the lines of each non-identity one.  ok[k]: 1 for a
+// valid encoding of a non-identity point, 2 for the identity, 0 for a rejected encoding.
+__global__ void k_g2_prepare(const uint8_t* enc, int count, LineCoeffs* lines, int* ok) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= count) return;
+  G2Affine q;
+  const bool valid = g2_decode(enc + 96 * k, &q);
+  ok[k] = !valid ? 0 : (q.inf ? 2 : 1);
+  if (valid && !q.inf) g2_prepare(q, lines + (size_t)PB_G2_LINES * k);
+}
+
+// e(P_k, Q_k) as an Fp12 (tests only); an identity on either side gives 1.
+__global__ void k_pairing_selftest(const uint4* g1, const LineCoeffs* lines, const int* ok, size_t n, uint32_t* out) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  G1Affine p[2] = {ld_aff(g1 + 6 * i), {Fp::zero(), Fp::zero()}};
+  if (ok[i] != 1) p[0] = p[1];
+  const LineCoeffs* l[2] = {lines + (size_t)PB_G2_LINES * i, lines};
+  const Fp12 f = final_exponentiation(miller_loop2(p, l));
+  const Fp* c = &f.c0.c0.c0;
+  for (int k = 0; k < 12; k++)
+    for (int j = 0; j < 12; j++) out[(i * 12 + k) * 12 + j] = c[k].v[j];
+}
+
+// ---- host side ------------------------------------------------------------------------------------------------
+std::once_flag g_consts_once;
+int g_consts_rc = 0;
+int upload_pairing_consts() {
+  std::call_once(g_consts_once, [] {
+    pairing_consts_init();
+    g_consts_rc = cudaMemcpyToSymbol(c_pairing, &h_pairing, sizeof h_pairing) == cudaSuccess ? 0 : 1;
+  });
+  return g_consts_rc ? fail(PB200_ERR_CUDA, "uploading the Frobenius coefficients") : 0;
+}
+
+// Decodes and prepares G2 points on the device: ok as k_g2_prepare, lines to d_lines (device).
+int g2_prepare_dev(const uint8_t* enc, int count, LineCoeffs* d_lines, int* ok, cudaStream_t st) {
+  PB_TRY(upload_pairing_consts());
+  uint8_t* d_enc = nullptr;
+  int* d_ok = nullptr;
+  PB_CUDA(cudaMallocAsync((void**)&d_enc, 96 * (size_t)count, st));
+  cudaError_t e = cudaMallocAsync((void**)&d_ok, sizeof(int) * count, st);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(d_enc, enc, 96 * (size_t)count, cudaMemcpyHostToDevice, st);
+  if (e == cudaSuccess) {
+    PB_LAUNCH(k_g2_prepare, div_up(count, 32), 32, 0, st, d_enc, count, d_lines, d_ok);
+    e = cudaGetLastError();
+  }
+  if (e == cudaSuccess) e = cudaMemcpyAsync(ok, d_ok, sizeof(int) * count, cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  cudaFreeAsync(d_enc, st);
+  if (d_ok) cudaFreeAsync(d_ok, st);
+  PB_CUDA(e);
+  return 0;
+}
+
+bool fr_canonical(const uint8_t* b, HFr* out) {  // BlsScalar::from_bytes: little-endian, below r
+  uint64_t w[4];
+  memcpy(w, b, 32);
+  for (int k = 3; k >= 0; k--) {
+    if (w[k] < pbh::kFrMod.p[k]) break;
+    if (w[k] > pbh::kFrMod.p[k] || k == 0) return false;
+  }
+  memcpy(out->v, w, 32);
+  *out = out->to_mont();
+  return true;
+}
+HFr fr_pow(HFr b, uint64_t e) {
+  HFr r = HFr::one();
+  for (; e; e >>= 1, b = b.sqr())
+    if (e & 1) r = r * b;
+  return r;
+}
+
+// Proof::verify up to the pairing: the transcript replay and the 32 scalars of k_verify_msm (canonical form).
+// Returns PB200_OK, PB200_ERR_POINT_MALFORMED for a non-canonical evaluation or PB200_ERR_VERIFY.
+int verify_scalars(const pb200_verifier* V, const uint8_t* proof, const HFr* pi, uint64_t* out) {
+  enum { A, B, C, D, AW, BW, DW, QARITH, QC, QL, QR, S1, S2, S3, Z };
+  HFr e[15];
+  for (int k = 0; k < 15; k++)
+    if (!fr_canonical(proof + 528 + 32 * k, &e[k])) return PB200_ERR_POINT_MALFORMED;
+  const uint8_t* cm = proof;  // a, b, c, d, z, t_low, t_mid, t_high, t_fourth, w_z, w_zw
+  pbh::Transcript tr = V->base;
+  for (size_t k = 0; k < V->pi_idx.size(); k++) tr.append_scalar("pi", pi[k]);
+  tr.append_commitment("a_comm", cm + 0);
+  tr.append_commitment("b_comm", cm + 48);
+  tr.append_commitment("c_comm", cm + 96);
+  tr.append_commitment("d_comm", cm + 144);
+  const HFr beta = tr.challenge_scalar("beta");
+  tr.append_scalar("beta", beta);
+  const HFr gamma = tr.challenge_scalar("gamma");
+  tr.append_commitment("z_comm", cm + 192);
+  const HFr alpha = tr.challenge_scalar("alpha");
+  const HFr ch_range = tr.challenge_scalar("range separation challenge");
+  const HFr ch_logic = tr.challenge_scalar("logic separation challenge");
+  const HFr ch_fixed = tr.challenge_scalar("fixed base separation challenge");
+  const HFr ch_var = tr.challenge_scalar("variable base separation challenge");
+  tr.append_commitment("t_low_comm", cm + 240);
+  tr.append_commitment("t_mid_comm", cm + 288);
+  tr.append_commitment("t_high_comm", cm + 336);
+  tr.append_commitment("t_fourth_comm", cm + 384);
+  const HFr z = tr.challenge_scalar("z_challenge");
+  tr.append_scalar("a_eval", e[A]); tr.append_scalar("b_eval", e[B]); tr.append_scalar("c_eval", e[C]); tr.append_scalar("d_eval", e[D]);
+  tr.append_scalar("s_sigma_1_eval", e[S1]); tr.append_scalar("s_sigma_2_eval", e[S2]); tr.append_scalar("s_sigma_3_eval", e[S3]);
+  tr.append_scalar("z_eval", e[Z]);
+  tr.append_scalar("a_w_eval", e[AW]); tr.append_scalar("b_w_eval", e[BW]); tr.append_scalar("d_w_eval", e[DW]);
+  tr.append_scalar("q_arith_eval", e[QARITH]); tr.append_scalar("q_c_eval", e[QC]); tr.append_scalar("q_l_eval", e[QL]); tr.append_scalar("q_r_eval", e[QR]);
+  const HFr v = tr.challenge_scalar("v_challenge");
+  const HFr v_w = tr.challenge_scalar("v_w_challenge");
+  tr.append_commitment("w_z_chall_comm", cm + 432);
+  tr.append_commitment("w_z_chall_w_comm", cm + 480);
+  const HFr u = tr.challenge_scalar("u_challenge");
+
+  const HFr one = HFr::one();
+  const HFr z_n = fr_pow(z, V->n), z_h = z_n - one;
+  // compute_lagrange_and_barycentric_evaluations (proof.rs:997-1040): one batch inversion
+  std::vector<HFr> den, pref;
+  std::vector<size_t> which;
+  den.push_back(V->size_fr * (z - one));
+  for (size_t k = 0; k < V->pi_idx.size(); k++)
+    if (!pi[k].is_zero()) {
+      den.push_back(V->pi_roots[k] * z - one);
+      which.push_back(k);
+    }
+  pref.resize(den.size());
+  HFr acc = one;
+  for (size_t k = 0; k < den.size(); k++) {
+    if (den[k].is_zero()) return PB200_ERR_VERIFY;
+    pref[k] = acc;
+    acc = acc * den[k];
+  }
+  HFr inv = acc.inv_bingcd();
+  for (size_t k = den.size(); k-- > 0;) {
+    const HFr d = den[k];
+    den[k] = inv * pref[k];
+    inv = inv * d;
+  }
+  const HFr l1 = z_h * den[0];
+  HFr pi_eval = HFr::zero();
+  for (size_t j = 0; j < which.size(); j++) pi_eval = pi_eval + den[1 + j] * pi[which[j]];
+  pi_eval = pi_eval * z_h * V->size_inv;
+
+  const HFr alpha_sq = alpha.sqr();
+  const HFr perm = (e[A] + beta * e[S1] + gamma) * (e[B] + beta * e[S2] + gamma) * (e[C] + beta * e[S3] + gamma);
+  const HFr r0 = pi_eval - l1 * alpha_sq - alpha * perm * (e[D] + gamma) * e[Z];
+  HFr vc[14];
+  vc[0] = v;
+  for (int k = 1; k < 11; k++) vc[k] = vc[k - 1] * v;
+  vc[11] = v_w * u;
+  vc[12] = vc[11] * v_w;
+  vc[13] = vc[12] * v_w;
+  const int eo[14] = {A, B, C, D, S1, S2, S3, QARITH, QC, QL, QR, AW, BW, DW};
+  HFr E = u * e[Z] - r0;
+  for (int k = 0; k < 14; k++) E = E + e[eo[k]] * vc[k];
+
+  // widget scalars (range, logic, fixed_base, curve_addition verifierkey.rs)
+  auto h4 = [](const HFr& x) { return x.dbl().dbl(); };
+  auto delta = [&](const HFr& f) { const HFr f1 = f - one, f2 = f1 - one, f3 = f2 - one; return f * f1 * f2 * f3; };
+  auto small = [](uint64_t k) { return HFr::from_u64(k); };
+  const HFr &a = e[A], &b = e[B], &c = e[C], &d = e[D], &a_w = e[AW], &b_w = e[BW], &d_w = e[DW];
+  HFr s_range, s_logic, s_fixed, s_var;
+  {
+    const HFr k = ch_range.sqr(), k2 = k.sqr(), k3 = k2 * k;
+    s_range = (delta(c - h4(d)) + delta(b - h4(c)) * k + delta(a - h4(b)) * k2 + delta(d_w - h4(a)) * k3) * ch_range;
+  }
+  {
+    const HFr k = ch_logic.sqr(), k2 = k.sqr(), k3 = k2 * k, k4 = k3 * k;
+    const HFr Aa = a_w - h4(a), Bb = b_w - h4(b), Dd = d_w - h4(d);
+    const HFr& w = c;
+    const HFr F = w * (w * (h4(w) - small(18) * (Aa + Bb) + small(81)) + small(18) * (Aa.sqr() + Bb.sqr()) - small(81) * (Aa + Bb) + small(83));
+    const HFr Ee = small(3) * (Aa + Bb + Dd) - F.dbl();
+    const HFr Bq = e[QC] * (small(9) * Dd - small(3) * (Aa + Bb));
+    s_logic = (delta(Aa) + delta(Bb) * k + delta(Dd) * k2 + (w - Aa * Bb) * k3 + (Bq + Ee) * k4) * ch_logic;
+  }
+  const HFr ed = (small(10240) * small(10241).inv()).neg();
+  {
+    const HFr k = ch_fixed.sqr(), k2 = k.sqr(), k3 = k2 * k;
+    const HFr bit = d_w - d - d;
+    const HFr bit_c = bit * (bit - one) * (bit + one);
+    const HFr y_alpha = bit.sqr() * (e[QR] - one) + one, x_alpha = bit * e[QL];
+    const HFr xy = (bit * e[QC] - c) * k;
+    const HFr t = c * a * b * ed;
+    const HFr xa = ((a_w + a_w * t) - (a * y_alpha + b * x_alpha)) * k2;
+    const HFr ya = ((b_w - b_w * t) - (b * y_alpha + a * x_alpha)) * k3;
+    s_fixed = (bit_c + xa + ya + xy) * ch_fixed;
+  }
+  {
+    const HFr k = ch_var.sqr();
+    const HFr xy = a * d - d_w, y1x2 = b * c, y1y2 = b * d, x1x2 = a * c;
+    const HFr t = ed * d_w * y1x2;
+    const HFr x3c = ((d_w + y1x2) - (a_w + a_w * t)) * k;
+    const HFr y3c = ((y1y2 + x1x2) - (b_w - b_w * t)) * k.sqr();
+    s_var = (xy + x3c + y3c) * ch_var;
+  }
+  // permutation verifierkey.rs
+  const HFr bz = beta * z;
+  const HFr xs = (a + bz + gamma) * (b + small(7) * bz + gamma) * (c + small(13) * bz + gamma) * (d + small(17) * bz + gamma) * alpha;
+  const HFr ys = perm * (beta * e[Z]) * alpha;
+  HFr f[11];
+  for (int k = 0; k < 11; k++) f[k] = vc[k];
+  f[0] = f[0] + vc[11];
+  f[1] = f[1] + vc[12];
+  f[3] = f[3] + vc[13];
+  const HFr qa = e[QARITH];
+  const HFr s[PB_VERIFY_TERMS] = {a * b * qa, a * qa, b * qa, c * qa, d * qa, qa, s_range, s_logic, s_fixed, s_var,
+                                  xs + l1 * alpha_sq + u, ys.neg(), z_h.neg(), z_n * z_h.neg(), z_n.sqr() * z_h.neg(),
+                                  z_n.sqr() * z_n * z_h.neg(), f[0], f[1], f[2], f[3], f[4], f[5], f[6], f[7], f[8], f[9], f[10],
+                                  E.neg(), z, u * z * V->group_gen, HFr::zero(), u};
+  for (int k = 0; k < PB_VERIFY_TERMS; k++) {
+    const HFr cn = s[k].from_mont();
+    memcpy(out + 4 * k, cn.v, 32);
+  }
+  return PB200_OK;
+}
+
+uint64_t be64(const uint8_t* b) {
+  uint64_t x = 0;
+  for (int k = 0; k < 8; k++) x = (x << 8) | b[k];
+  return x;
+}
+void put_be64(std::vector<uint8_t>& o, uint64_t x) {
+  for (int k = 7; k >= 0; k--) o.push_back((uint8_t)(x >> (8 * k)));
+}
+
+// VerifierKey::to_bytes (widget.rs:84-111) orders the commitments q_m, q_l, q_r, q_o, q_f, q_c, q_arith, q_logic,
+// q_range, q_fixed_group_add, q_variable_group_add, s_sigma_1..4; pb200_prover_commitments has q_range before q_logic.
+const int kFileOrder[15] = {0, 1, 2, 3, 4, 5, 6, 8, 7, 9, 10, 11, 12, 13, 14};
+constexpr size_t kVerifierKeyBytes = 20 * 48 + 8;
+
+// Verifier::new (verifier.rs:32-60) from validated parts.  vk_n is VerifierKey::n, which Compiler::compile sets to the
+// constraint count (compiler.rs:278-279); the domain is EvaluationDomain::new(vk_n).
+int verifier_build(const uint8_t* label, size_t label_len, uint64_t vk_n, uint64_t size, uint64_t constraints, const uint8_t* comms,
+                   const uint8_t* opening_key, const uint64_t* pi_idx, size_t n_pi, pb200_verifier** out) {
+  PB_TRY(ensure_init());
+  // the 15 commitments and opening_key.g: checked decoding (Commitment / G1Affine::from_bytes)
+  std::vector<uint8_t> enc(16 * 48), raw(16 * 96);
+  memcpy(enc.data(), comms, 15 * 48);
+  memcpy(enc.data() + 15 * 48, opening_key, 48);
+  PB_TRY(g1_decompress(enc.data(), 16, 1, raw.data()));
+  bool g_inf = true;
+  for (int k = 0; k < 96; k++) g_inf = g_inf && raw[15 * 96 + k] == 0;
+  cudaStream_t st = thread_stream();
+  LineCoeffs* d_lines = nullptr;
+  PB_CUDA(cudaMalloc((void**)&d_lines, 2 * PB_G2_LINES * sizeof(LineCoeffs)));
+  uint8_t g2[2 * 96];
+  memcpy(g2, opening_key + 48 + 96, 96);  // [x]H first: the pair of -(W_z + u W_zw)
+  memcpy(g2 + 96, opening_key + 48, 96);
+  int ok[2] = {0, 0};
+  int rc = g2_prepare_dev(g2, 2, d_lines, ok, st);
+  if (rc == 0 && (g_inf || ok[0] != 1 || ok[1] != 1))
+    rc = fail(PB200_ERR_POINT_MALFORMED, "InvalidData: opening key point is the identity, not on the curve or not in the subgroup");
+  // EvaluationDomain::new (domain.rs:118-160)
+  int log_n = 0;
+  while (rc == 0 && log_n < 64 && ((uint64_t)1 << log_n) < vk_n) log_n++;
+  if (rc == 0 && log_n >= 32) rc = fail(PB200_ERR_INVALID_DOMAIN, "InvalidEvalDomainSize");
+  if (rc) {
+    cudaFree(d_lines);
+    return rc;
+  }
+  pb200_verifier* V = new pb200_verifier();
+  V->d_lines = d_lines;
+  V->label.assign(label, label + label_len);
+  V->vk_n = vk_n;
+  V->n = (uint64_t)1 << log_n;
+  V->size = size;
+  V->constraints = constraints;
+  memcpy(V->vk_comm, comms, 15 * 48);
+  memcpy(V->opening_key, opening_key, PB200_OPENING_KEY_BYTES);
+  V->pi_idx.assign(pi_idx, pi_idx + n_pi);
+  // ROOT_OF_UNITY = 7^((r - 1) / 2^32), squared down to the domain
+  uint64_t t[4];
+  memcpy(t, pbh::kFrMod.p, 32);
+  t[0] -= 1;
+  for (int k = 0; k < 4; k++) t[k] = (t[k] >> 32) | (k < 3 ? t[k + 1] << 32 : 0);
+  HFr g = HFr::from_u64(7).pow(t, 4);
+  for (int k = log_n; k < 32; k++) g = g.sqr();
+  V->group_gen = g;
+  V->size_fr = HFr::from_u64(V->n);
+  V->size_inv = V->size_fr.inv();
+  const HFr g_inv = g.inv();
+  for (uint64_t idx : V->pi_idx) V->pi_roots.push_back(fr_pow(g_inv, idx));
+  // Transcript::base (transcript.rs:131-145) with VerifierKey::seed_transcript (widget.rs:218-257)
+  V->base = pbh::Transcript(V->label.data(), V->label.size());
+  V->base.circuit_domain_sep(constraints);
+  static const char* lbl[15] = {"q_m", "q_l", "q_r", "q_o", "q_c", "q_f", "q_arith", "q_range", "q_logic",
+                                "q_variable_group_add", "q_fixed_group_add", "s_sigma_1", "s_sigma_2", "s_sigma_3", "s_sigma_4"};
+  static const int ord[15] = {0, 1, 2, 3, 5, 4, 6, 7, 8, 10, 9, 11, 12, 13, 14};
+  for (int k = 0; k < 15; k++) V->base.append_commitment(lbl[k], comms + 48 * ord[k]);
+  V->base.circuit_domain_sep(vk_n);  // seed_transcript_inner ends with VerifierKey::n (widget.rs:256)
+  cudaError_t e = cudaMalloc((void**)&V->d_points, 16 * 96);
+  if (e == cudaSuccess) e = cudaMemcpy(V->d_points, raw.data(), 16 * 96, cudaMemcpyHostToDevice);
+  if (e != cudaSuccess) {
+    cudaFree(V->d_points);
+    cudaFree(V->d_lines);
+    delete V;
+    return fail(PB200_ERR_CUDA, "verifier key upload", cudaGetErrorString(e));
+  }
+  *out = V;
+  return 0;
+}
+
+}  // namespace
+}  // namespace pb
+
+using namespace pb;
+
+extern "C" {
+
+int pb200_verifier_new(const uint8_t* label, size_t label_len, size_t n_constraints, const uint8_t* vk_comms_15x48,
+                       const uint8_t* opening_key, const uint64_t* pi_idx, size_t n_pi, pb200_verifier_t** out) {
+  if ((!label && label_len) || !vk_comms_15x48 || !opening_key || (!pi_idx && n_pi) || !out) return fail(PB200_ERR_INVALID_ARG, "null argument");
+  uint64_t size = 1;  // Verifier::size = constraints.next_power_of_two() (compiler.rs:141)
+  while (size < n_constraints && size) size <<= 1;
+  if (!size) return fail(PB200_ERR_INVALID_DOMAIN, "InvalidEvalDomainSize");
+  return verifier_build(label, label_len, n_constraints, size, n_constraints, vk_comms_15x48, opening_key, pi_idx, n_pi, out);
+}
+
+int pb200_verifier_from_bytes(const uint8_t* bytes, size_t len, pb200_verifier_t** out) {
+  if (!bytes || !out) return fail(PB200_ERR_INVALID_ARG, "null argument");
+  if (len < 48) return fail(PB200_ERR_INVALID_ARG, "NotEnoughBytes");
+  const uint64_t label_len = be64(bytes), vk_len = be64(bytes + 8), ok_len = be64(bytes + 16), n_pi = be64(bytes + 24);
+  const uint64_t size = be64(bytes + 32), constraints = be64(bytes + 40);
+  // checked arithmetic as verifier.rs:150-165: any overflow is NotEnoughBytes
+  if (n_pi > UINT64_MAX / 8) return fail(PB200_ERR_INVALID_ARG, "NotEnoughBytes");
+  uint64_t need = label_len;
+  for (uint64_t add : {vk_len, ok_len, n_pi * 8}) {
+    if (need > UINT64_MAX - add) return fail(PB200_ERR_INVALID_ARG, "NotEnoughBytes");
+    need += add;
+  }
+  if (len - 48 < need) return fail(PB200_ERR_INVALID_ARG, "NotEnoughBytes");
+  const uint8_t* p = bytes + 48;
+  const uint8_t* label = p;
+  const uint8_t* vk = label + label_len;
+  const uint8_t* okey = vk + vk_len;
+  const uint8_t* pis = okey + ok_len;
+  // VerifierKey::from_slice / OpeningKey::from_slice read exactly their sizes
+  if (vk_len < kVerifierKeyBytes || ok_len < PB200_OPENING_KEY_BYTES) return fail(PB200_ERR_INVALID_ARG, "BadLength");
+  uint64_t n = 0;
+  for (int k = 7; k >= 0; k--) n = (n << 8) | vk[k];
+  uint8_t comms[15 * 48];
+  for (int k = 0; k < 15; k++) memcpy(comms + 48 * k, vk + 8 + 48 * k, 48);
+  uint8_t ordered[15 * 48];
+  for (int k = 0; k < 15; k++) memcpy(ordered + 48 * kFileOrder[k], comms + 48 * k, 48);
+  std::vector<uint64_t> idx(n_pi);
+  for (uint64_t k = 0; k < n_pi; k++) idx[k] = be64(pis + 8 * k);
+  return verifier_build(label, label_len, n, size, constraints, ordered, okey, idx.data(), idx.size(), out);
+}
+
+int pb200_verifier_to_bytes(const pb200_verifier_t* V, uint8_t* out, size_t cap, size_t* len) {
+  if (!V || !len) return fail(PB200_ERR_INVALID_ARG, "null argument");
+  std::vector<uint8_t> o;
+  put_be64(o, V->label.size());
+  put_be64(o, kVerifierKeyBytes);
+  put_be64(o, PB200_OPENING_KEY_BYTES);
+  put_be64(o, V->pi_idx.size());
+  put_be64(o, V->size);
+  put_be64(o, V->constraints);
+  o.insert(o.end(), V->label.begin(), V->label.end());
+  const size_t vk_at = o.size();
+  for (int k = 0; k < 8; k++) o.push_back((uint8_t)(V->vk_n >> (8 * k)));
+  for (int k = 0; k < 15; k++) o.insert(o.end(), V->vk_comm[kFileOrder[k]], V->vk_comm[kFileOrder[k]] + 48);
+  o.resize(vk_at + kVerifierKeyBytes, 0);
+  o.insert(o.end(), V->opening_key, V->opening_key + PB200_OPENING_KEY_BYTES);
+  for (uint64_t i : V->pi_idx) put_be64(o, i);
+  *len = o.size();
+  if (!out) return 0;
+  if (cap < o.size()) return fail(PB200_ERR_INVALID_ARG, "output buffer too small");
+  memcpy(out, o.data(), o.size());
+  return 0;
+}
+
+void pb200_verifier_free(pb200_verifier_t* V) {
+  if (!V) return;
+  ensure_init();
+  cudaFree(V->d_points);
+  cudaFree(V->d_lines);
+  delete V;
+}
+
+int pb200_verify(const pb200_verifier_t* V, const uint8_t* proofs, size_t n_proofs, const uint64_t* pi_vals, size_t n_pi,
+                 int32_t* status) {
+  PB_TRY(ensure_init());
+  if (!V || (!proofs && n_proofs) || (!pi_vals && n_pi && n_proofs) || (!status && n_proofs)) return fail(PB200_ERR_INVALID_ARG, "null argument");
+  if (n_pi != V->pi_idx.size()) return fail(PB200_ERR_INVALID_ARG, "InconsistentPublicInputsLen");
+  if (!n_proofs) return 0;
+  PB_TRY(upload_pairing_consts());
+  // host: transcripts and scalars, spread over threads for large batches
+  std::vector<uint64_t> scal(n_proofs * PB_VERIFY_TERMS * 4);
+  std::vector<int> hstat(n_proofs);
+  std::vector<uint8_t> comm(n_proofs * 528);
+  auto work = [&](size_t lo, size_t hi) {
+    for (size_t i = lo; i < hi; i++) {
+      const uint8_t* pr = proofs + 1008 * i;
+      memcpy(comm.data() + 528 * i, pr, 528);
+      hstat[i] = verify_scalars(V, pr, (const HFr*)(pi_vals + 4 * n_pi * i), scal.data() + (size_t)PB_VERIFY_TERMS * 4 * i);
+    }
+  };
+  const size_t n_thr = std::min<size_t>(std::max(1u, std::thread::hardware_concurrency()), std::min<size_t>(16, (n_proofs + 31) / 32));
+  if (n_thr <= 1) {
+    work(0, n_proofs);
+  } else {
+    std::vector<std::thread> th;
+    const size_t per = (n_proofs + n_thr - 1) / n_thr;
+    for (size_t t = 0; t < n_thr; t++) th.emplace_back(work, std::min(n_proofs, t * per), std::min(n_proofs, (t + 1) * per));
+    for (auto& x : th) x.join();
+  }
+  // device: decoding, the two G1 points, the pairing check
+  cudaStream_t st = thread_stream();
+  ScratchScope scope(nullptr, st);
+  uint8_t* d_comm;
+  uint4 *d_pts, *d_scal, *d_g1;
+  unsigned* d_bad;
+  int* d_stat;
+  PB_ALLOC(scope, d_comm, n_proofs * 528);
+  PB_ALLOC(scope, d_pts, n_proofs * 11 * 96);
+  PB_ALLOC(scope, d_scal, scal.size() * 8);
+  PB_ALLOC(scope, d_g1, n_proofs * 2 * 96);
+  PB_ALLOC(scope, d_bad, 4);
+  PB_ALLOC(scope, d_stat, n_proofs * sizeof(int));
+  PB_CUDA(cudaMemcpyAsync(d_comm, comm.data(), n_proofs * 528, cudaMemcpyHostToDevice, st));
+  PB_CUDA(cudaMemcpyAsync(d_scal, scal.data(), scal.size() * 8, cudaMemcpyHostToDevice, st));
+  PB_CUDA(cudaMemcpyAsync(d_stat, hstat.data(), n_proofs * sizeof(int), cudaMemcpyHostToDevice, st));
+  g1_decompress_dev(d_comm, n_proofs * 11, d_pts, d_bad, st);
+  PB_LAUNCH(k_verify_msm, div_up(n_proofs * 32, 128), 128, 0, st, V->d_points, d_pts, d_comm, d_scal, n_proofs, d_stat, d_g1);
+  PB_LAUNCH(k_verify_pairing, div_up(n_proofs, 64), 64, 0, st, d_g1, V->d_lines, n_proofs, d_stat);
+  PB_CUDA(cudaGetLastError());
+  PB_CUDA(cudaMemcpyAsync(hstat.data(), d_stat, n_proofs * sizeof(int), cudaMemcpyDeviceToHost, st));
+  PB_CUDA(cudaStreamSynchronize(st));
+  for (size_t i = 0; i < n_proofs; i++) status[i] = hstat[i];
+  return 0;
+}
+
+int pb200_selftest_pairing(const uint64_t* g1_raw, const uint8_t* g2_compressed, size_t n, uint64_t* out_fp12) {
+  PB_TRY(ensure_init());
+  if (!n) return 0;
+  if (!g1_raw || !g2_compressed || !out_fp12) return fail(PB200_ERR_INVALID_ARG, "null argument");
+  cudaStream_t st = thread_stream();
+  ScratchScope scope(nullptr, st);
+  LineCoeffs* d_lines;
+  uint4* d_g1;
+  int* d_ok;
+  uint32_t* d_out;
+  PB_ALLOC(scope, d_lines, n * PB_G2_LINES * sizeof(LineCoeffs));
+  PB_ALLOC(scope, d_g1, n * 96);
+  PB_ALLOC(scope, d_ok, n * sizeof(int));
+  PB_ALLOC(scope, d_out, n * 576);
+  std::vector<int> ok(n);
+  PB_TRY(g2_prepare_dev(g2_compressed, (int)n, d_lines, ok.data(), st));
+  for (size_t i = 0; i < n; i++)
+    if (!ok[i]) return fail(PB200_ERR_POINT_MALFORMED, "malformed G2 encoding");
+  PB_CUDA(cudaMemcpyAsync(d_ok, ok.data(), n * sizeof(int), cudaMemcpyHostToDevice, st));
+  PB_CUDA(cudaMemcpyAsync(d_g1, g1_raw, n * 96, cudaMemcpyHostToDevice, st));
+  PB_LAUNCH(k_pairing_selftest, div_up(n, 32), 32, 0, st, d_g1, d_lines, d_ok, n, d_out);
+  PB_CUDA(cudaGetLastError());
+  PB_CUDA(cudaMemcpyAsync(out_fp12, d_out, n * 576, cudaMemcpyDeviceToHost, st));
+  PB_CUDA(cudaStreamSynchronize(st));
+  return 0;
+}
+}

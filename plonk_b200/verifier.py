@@ -1,0 +1,82 @@
+"""Verifier (reference src/compiler/verifier.rs, PlonkVersion::V3) on the GPU, through pb200_verifier_* and
+pb200_verify of include/plonk_b200.h."""
+from __future__ import annotations
+
+import ctypes
+from typing import List, Sequence
+
+from ._lib import PB200_ERR_INVALID_ARG, PB200_ERR_POINT_MALFORMED, PB200_ERR_VERIFY, Pb200Error, check, lib
+
+PROOF_BYTES = 1008
+OPENING_KEY_BYTES = 240
+
+
+class ProofVerificationError(Exception):
+    """Error::ProofVerificationError: the proof does not satisfy the verifier's equation."""
+
+
+class PointMalformed(Exception):
+    """dusk_bytes InvalidData from Proof::from_bytes: a malformed commitment or a non-canonical scalar."""
+
+
+class Verifier:
+    def __init__(self, label: bytes, n_constraints: int, commitments: Sequence[bytes], opening_key: bytes, pi_idx: bytes = b""):
+        """commitments: the 15 compressed verifier-key commitments in Prover.commitments() order; opening_key:
+        OpeningKey::to_bytes; pi_idx: public-input positions as little-endian u64 (as Prover.prove takes them)."""
+        assert len(commitments) == 15 and len(opening_key) == OPENING_KEY_BYTES and len(pi_idx) % 8 == 0
+        h = ctypes.c_void_p()
+        check(lib().pb200_verifier_new(label, len(label), n_constraints, b"".join(commitments), opening_key, pi_idx or None,
+                                       len(pi_idx) // 8, ctypes.byref(h)))
+        self._h = h
+        self.n_pi = len(pi_idx) // 8
+
+    @classmethod
+    def from_bytes(cls, data: bytes) -> "Verifier":
+        """Verifier::try_from_bytes."""
+        self = cls.__new__(cls)
+        h = ctypes.c_void_p()
+        check(lib().pb200_verifier_from_bytes(data, len(data), ctypes.byref(h)))
+        self._h = h
+        self.n_pi = int.from_bytes(data[24:32], "big")
+        return self
+
+    def to_bytes(self) -> bytes:
+        """Verifier::to_bytes."""
+        n = ctypes.c_size_t()
+        check(lib().pb200_verifier_to_bytes(self._h, None, 0, ctypes.byref(n)))
+        out = ctypes.create_string_buffer(n.value)
+        check(lib().pb200_verifier_to_bytes(self._h, out, n.value, ctypes.byref(n)))
+        return out.raw
+
+    def verify_batch(self, proofs: Sequence[bytes], pi_vals: Sequence[bytes]) -> List[int]:
+        """One status per proof (PB200_OK, PB200_ERR_VERIFY or PB200_ERR_POINT_MALFORMED); pi_vals[i]: the public
+        inputs of proof i, 32 bytes (Montgomery form) each."""
+        assert len(proofs) == len(pi_vals) and all(len(p) == PROOF_BYTES for p in proofs)
+        n_pi = len(pi_vals[0]) // 32 if pi_vals else self.n_pi
+        if any(len(v) != 32 * n_pi for v in pi_vals):
+            raise ValueError("every proof needs the same number of public inputs")
+        status = (ctypes.c_int32 * max(1, len(proofs)))()
+        vals = b"".join(pi_vals)
+        check(lib().pb200_verify(self._h, b"".join(proofs), len(proofs), vals or None, n_pi, status))
+        return list(status[: len(proofs)])
+
+    def verify(self, proof: bytes, pi_vals: bytes) -> None:
+        """Verifier::verify: returns on success, raises ProofVerificationError, PointMalformed or ValueError."""
+        try:
+            (st,) = self.verify_batch([proof], [pi_vals])
+        except Pb200Error as e:
+            if e.code == PB200_ERR_INVALID_ARG:
+                raise ValueError(str(e)) from e
+            raise
+        if st == PB200_ERR_VERIFY:
+            raise ProofVerificationError("ProofVerificationError")
+        if st == PB200_ERR_POINT_MALFORMED:
+            raise PointMalformed("InvalidData")
+
+    def __del__(self):
+        try:
+            if getattr(self, "_h", None):
+                lib().pb200_verifier_free(self._h)
+                self._h = None
+        except Exception:
+            pass
