@@ -70,11 +70,6 @@ Fr fr_recompose(const uint8_t bits[256], int start, int end) {
 // ---------------------------------------------------------------------------------------------
 const uint64_t kJubJubOrder[4] = {0xd0970e5ed6f72cb7ull, 0xa6682093ccc81082ull, 0x06673b0101343b00ull, 0x0e7db4ea6533afa9ull};
 
-const Fr& edwards_d() {
-  static const Fr d = (fr_u64(10240) * fr_u64(10241).inv_bingcd()).neg();
-  return d;
-}
-
 JubJubAffine jj_identity() { return {Fr::zero(), Fr::one()}; }
 
 JubJubAffine jj_generator() {

@@ -53,7 +53,7 @@ JubJubAffine jj_neg(const JubJubAffine& p);
 JubJubAffine jj_mul(const JubJubAffine& p, const uint64_t k[4]);  // canonical little-endian scalar
 bool jj_is_on_curve(const JubJubAffine& p);
 bool jj_is_torsion_free(const JubJubAffine& p);
-const Fr& edwards_d();
+using pbh::edwards_d;
 extern const uint64_t kJubJubOrder[4];
 
 // One width-4 gate being built: selector coefficients, optional public input, four wires.

@@ -115,6 +115,12 @@ struct HField {
       }
     return acc;
   }
+  HField pow_u64(uint64_t e) const {  // from the low bit: as many squarings as e has bits
+    HField acc = one(), b = *this;
+    for (; e; e >>= 1, b = b.sqr())
+      if (e & 1) acc = acc * b;
+    return acc;
+  }
   HField inv() const {  // Fermat; 0 -> 0
     uint64_t e[N];
     memcpy(e, M.p, sizeof e);
@@ -227,6 +233,12 @@ extern const Mod64<6> kFpMod;
 extern const Mod64<4> kFrMod;
 typedef HField<6, kFpMod> HFp;
 typedef HField<4, kFrMod> HFr;
+
+// dusk_jubjub::EDWARDS_D = -(10240 / 10241), Montgomery form
+inline const HFr& edwards_d() {
+  static const HFr d = (HFr::from_u64(10240) * HFr::from_u64(10241).inv_bingcd()).neg();
+  return d;
+}
 
 // G1 in XYZZ coordinates on the host (same formulas as csrc/g1.cuh).
 struct HXyzz {

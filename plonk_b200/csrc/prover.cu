@@ -23,6 +23,7 @@
 
 #include "common.cuh"
 #include "host_field.h"
+#include "plonk_algebra.cuh"
 #include "transcript.h"
 
 struct pb200_srs;
@@ -53,8 +54,6 @@ int fill_powers(uint4* out, size_t n, const Fr& base, const Fr& scale, cudaStrea
 Fr ntt_group_gen(int log_n, bool inverse);
 Fr ntt_size_inv(int log_n);
 Fr ntt_coset_gen(bool inverse);
-
-enum { Q_M, Q_L, Q_R, Q_O, Q_F, Q_C, Q_ARITH, Q_RANGE, Q_LOGIC, Q_FIXED, Q_VAR, S1, S2, S3, S4, N_POLY };
 
 PB_D Fr ldg_fr(const uint4* p, size_t i) {
   uint4 a = __ldg(p + 2 * i), b = __ldg(p + 2 * i + 1);
@@ -271,10 +270,6 @@ __global__ void k_scan_fixup(uint4* out, size_t n, const uint4* block_prefix) {
 // ---------------------------------------------------------------------------------------------
 // Quotient numerator on the 8n coset (quotient_poly.rs:160-310 + all widget compute_quotient_i)
 // ---------------------------------------------------------------------------------------------
-struct WidgetCh {
-  Fr ch, k, k2, k3, k4;
-};
-
 struct QuotArgs {
   const uint4* w8;      // [6][8n]: z, a, b, c, d, pi coset evaluations
   const uint4* key8;    // [15][8n] prover-key coset evaluations (enum order)
@@ -285,7 +280,7 @@ struct QuotArgs {
   Fr alpha, beta, gamma, alpha_sq;
   // separation challenges with their powers (kappa = ch^2, kappa^2, ...), computed once on the host
   // instead of once per coset point
-  WidgetCh ch_range, ch_logic, ch_fixed, ch_var;
+  SepPowers<Fr> ch_range, ch_logic, ch_fixed, ch_var;
   Fr edwards_d;  // dusk_jubjub::EDWARDS_D, Montgomery form
   Fr vh_inv[8];
   int has_range, has_logic, has_fixed, has_var;
@@ -311,65 +306,6 @@ struct Q {
   PB_D Q dbl() const { return Q(v.dbl()); }
 };
 
-template <class F>
-PB_D F delta4(const F& f) {  // f (f - 1)(f - 2)(f - 3) = g (g + 2) with g = f (f - 3): two products
-  const F one = F::one();
-  const F g = f * (f - one - one - one);
-  return g * (g + one + one);
-}
-template <class F>
-PB_D F mul_small(const F& x, int k) {  // k * x for small positive k by additions
-  F acc = F::zero(), p = x;
-  while (k) {
-    if (k & 1) acc = acc + p;
-    p = p.dbl();
-    k >>= 1;
-  }
-  return acc;
-}
-
-struct WireVals {
-  Q a, b, c, d, a_w, b_w, d_w;
-};
-PB_D Q widget_range(const WidgetCh& s, const WireVals& v) {  // range/proverkey.rs:32-57 (without selector)
-  const Q &ch = s.ch, &k = s.k, &k2 = s.k2, &k3 = s.k3;
-  Q t = delta4(v.c - mul_small(v.d, 4)) + delta4(v.b - mul_small(v.c, 4)) * k + delta4(v.a - mul_small(v.b, 4)) * k2 +
-         delta4(v.d_w - mul_small(v.a, 4)) * k3;
-  return t * ch;
-}
-PB_D Q widget_logic(const WidgetCh& s, const Q& q_c, const WireVals& v) {  // logic/proverkey.rs:34-71, 120-144
-  const Q &ch = s.ch, &k = s.k, &k2 = s.k2, &k3 = s.k3, &k4 = s.k4;
-  Q A = v.a_w - mul_small(v.a, 4), B = v.b_w - mul_small(v.b, 4), D = v.d_w - mul_small(v.d, 4);
-  const Q& w = v.c;
-  Q ab = A + B;
-  Q F = w * (w * (mul_small(w, 4) - mul_small(ab, 18) + mul_small(Q::one(), 81)) + mul_small(A.sqr() + B.sqr(), 18) - mul_small(ab, 81) + mul_small(Q::one(), 83));
-  Q E = mul_small(ab + D, 3) - F.dbl();
-  Q Bq = q_c * (mul_small(D, 9) - mul_small(ab, 3));
-  Q t = delta4(A) + delta4(B) * k + delta4(D) * k2 + (w - A * B) * k3 + (Bq + E) * k4;
-  return t * ch;
-}
-PB_D Q widget_fixed(const WidgetCh& s, const Q& ed, const Q& q_l, const Q& q_r, const Q& q_c, const WireVals& v) {  // fixed_base/proverkey.rs:39-103
-  const Q one = Q::one();
-  const Q &ch = s.ch, &k = s.k, &k2 = s.k2, &k3 = s.k3;
-  Q bit = v.d_w - v.d - v.d;
-  Q bit_c = bit * (bit - one) * (bit + one);
-  Q y_alpha = bit.sqr() * (q_r - one) + one, x_alpha = bit * q_l;
-  Q xy = (bit * q_c - v.c) * k;
-  Q t = v.c * v.a * v.b * ed;
-  Q xa = ((v.a_w + v.a_w * t) - (v.a * y_alpha + v.b * x_alpha)) * k2;
-  Q ya = ((v.b_w - v.b_w * t) - (v.b * y_alpha + v.a * x_alpha)) * k3;
-  return (bit_c + xa + ya + xy) * ch;
-}
-PB_D Q widget_var(const WidgetCh& s, const Q& ed, const WireVals& v) {  // curve_addition/proverkey.rs:33-79
-  const Q &ch = s.ch, &k = s.k;
-  const Q &x1 = v.a, &x3 = v.a_w, &y1 = v.b, &y3 = v.b_w, &x2 = v.c, &y2 = v.d, &x1y2 = v.d_w;
-  Q xy = x1 * y2 - x1y2, y1x2 = y1 * x2, y1y2 = y1 * y2, x1x2 = x1 * x2;
-  Q t = ed * x1y2 * y1x2;
-  Q x3c = ((x1y2 + y1x2) - (x3 + x3 * t)) * k;
-  Q y3c = ((y1y2 + x1x2) - (y3 - y3 * t)) * s.k2;
-  return (xy + x3c + y3c) * ch;
-}
-
 // One point of the quotient.  The six witness rows (z, a, b, c, d, pi) have stride `ws` and are read at
 // column i, the "next row" values (X -> omega X) at column iw; the prover-key tables (stride n8),
 // the point itself, L_1 and 1/Z_H are read at index ki of the 8n coset; the result goes to out[oi].
@@ -378,7 +314,7 @@ PB_D Q widget_var(const WidgetCh& s, const Q& ed, const WireVals& v) {  // curve
 //   single points (Horner-evaluated):    ws = 16, iw = i + 8,        ki = 1 + n i, oi = i
 PB_D void quotient_point(const QuotArgs& q, size_t ws, size_t i, size_t iw, size_t ki, size_t oi) {
   const size_t n8 = q.n8;
-  WireVals v;
+  WireVals<Q> v;
   const Q z = ldg_fr(q.w8, i), z_w = ldg_fr(q.w8, iw);
   v.a = ldg_fr(q.w8, ws + i); v.a_w = ldg_fr(q.w8, ws + iw);
   v.b = ldg_fr(q.w8, 2 * ws + i); v.b_w = ldg_fr(q.w8, 2 * ws + iw);
@@ -391,17 +327,15 @@ PB_D void quotient_point(const QuotArgs& q, size_t ws, size_t i, size_t iw, size
   Q t = (v.a * v.b * KEY(Q_M) + v.a * q_l + v.b * q_r + v.c * KEY(Q_O) + v.d * KEY(Q_F) + q_c) * KEY(Q_ARITH);
   if (q.has_range) t = t + widget_range(q.ch_range, v) * KEY(Q_RANGE);
   if (q.has_logic) t = t + widget_logic(q.ch_logic, q_c, v) * KEY(Q_LOGIC);
-  if (q.has_fixed) t = t + widget_fixed(q.ch_fixed, q.edwards_d, q_l, q_r, q_c, v) * KEY(Q_FIXED);
-  if (q.has_var) t = t + widget_var(q.ch_var, q.edwards_d, v) * KEY(Q_VAR);
+  if (q.has_fixed) t = t + widget_fixed(q.ch_fixed, Q(q.edwards_d), q_l, q_r, q_c, v) * KEY(Q_FIXED);
+  if (q.has_var) t = t + widget_var(q.ch_var, Q(q.edwards_d), v) * KEY(Q_VAR);
   t = t + pi;
   // permutation/proverkey.rs:40-125
   const Q x = ldg_fr(q.linear8, ki);
   const Q alpha = q.alpha, beta = q.beta, gamma = q.gamma;
   const Q bx = beta * x;
-  Q ident = (v.a + bx + gamma) * (v.b + mul_small(bx, 7) + gamma) * (v.c + mul_small(bx, 13) + gamma) *
-            (v.d + mul_small(bx, 17) + gamma) * z * alpha;
-  Q copy = (v.a + beta * KEY(S1) + gamma) * (v.b + beta * KEY(S2) + gamma) * (v.c + beta * KEY(S3) + gamma) *
-           (v.d + beta * KEY(S4) + gamma) * z_w * alpha;
+  Q ident = perm_ident(v, bx, gamma) * z * alpha;
+  Q copy = perm_copy3(v, beta, gamma, [&](int j) { return Q(KEY(S1 + j)); }) * (v.d + beta * KEY(S4) + gamma) * z_w * alpha;
 #undef KEY
   Q l1 = Q(ldg_fr(q.l1_8, ki)) * Q(q.alpha_sq);
   t = t + ident - copy + (z - Q::one()) * l1;
@@ -640,7 +574,6 @@ static HFr to_host(const Fr& x) {
   memcpy(r.v, x.v, 32);
   return r;
 }
-static HFr hfr_pow(const HFr& x, uint64_t e) { return x.pow(&e, 1); }
 
 // Exclusive scan of n elements: CTA-local scans of 2048 elements, the scan of the CTA totals (by the same
 // routine, so any length works: 2^22 + 8 elements are 2049 totals, two levels), then the fix-up.
@@ -824,7 +757,7 @@ static int prover_build(pb200_prover* P, const uint8_t* label, size_t label_len,
   // (prover.rs:78-91).  L_1 on the coset: vh[i] * (8 / 8n) / (x_i - 1)  (quotient_poly.rs:265-284).
   {
     const HFr g = to_host(ntt_coset_gen(false)), w8n = to_host(ntt_group_gen(log_n + 3, false));
-    HFr point = hfr_pow(g, n), step = hfr_pow(w8n, n);
+    HFr point = g.pow_u64(n), step = w8n.pow_u64(n);
     const HFr psi = to_host(ntt_size_inv(log_n + 3)) * HFr::from_u64(8);
     Period8 c;
     for (int i = 0; i < 8; i++) {
@@ -839,10 +772,9 @@ static int prover_build(pb200_prover* P, const uint8_t* label, size_t label_len,
     PB_LAUNCH(k_scale_period8, div_up(n8, 256), 256, 0, st, P->d_l1_8, n8, c);
   }
   {  // per-domain constants of round 3, computed once (each costs a host-side inversion or power)
-    P->edwards_d = to_dev((HFr::from_u64(10240) * HFr::from_u64(10241).inv()).neg());
+    P->edwards_d = to_dev(pbh::edwards_d());
     const HFr g = to_host(ntt_coset_gen(false)), w8n = to_host(ntt_group_gen(log_n + 3, false));
-    const uint64_t e_n[1] = {(uint64_t)n}, e_4n[1] = {(uint64_t)(4 * n)};
-    const HFr h = g * w8n, w8r = w8n.pow(e_n, 1), wn = to_host(ntt_group_gen(log_n, false)), g4n = g.pow(e_4n, 1);
+    const HFr h = g * w8n, w8r = w8n.pow_u64(n), wn = to_host(ntt_group_gen(log_n, false)), g4n = g.pow_u64(4 * n);
     HFr xs[16];
     xs[0] = h;
     for (int k = 1; k < 8; k++) xs[k] = xs[k - 1] * w8r;
@@ -915,8 +847,7 @@ int prover_from_bytes(const uint8_t* bytes, size_t len, const uint32_t* wires, s
   const uint8_t* pk = label + label_len;
   const uint8_t* ck = pk + pk_len;
   const uint8_t* vk = ck + ck_len;
-  // ProverKey::to_var_bytes (widget.rs:347-445); file order of the 15 polynomials -> this file's enum
-  static const int file_order[N_POLY] = {Q_M, Q_L, Q_R, Q_O, Q_F, Q_C, Q_ARITH, Q_LOGIC, Q_RANGE, Q_FIXED, Q_VAR, S1, S2, S3, S4};
+  // ProverKey::to_var_bytes (widget.rs:347-445)
   LoadedProverKey key;
   {
     size_t off = 0;
@@ -932,8 +863,8 @@ int prover_from_bytes(const uint8_t* bytes, size_t len, const uint32_t* wires, s
       off += 8;
       if (cnt > n) return fail(bad_rc, "InvalidData: polynomial longer than the domain");
       if (!need(cnt * 32)) return fail(short_rc, "NotEnoughBytes: prover key polynomial");
-      key.poly[file_order[i]] = pk + off;
-      key.poly_len[file_order[i]] = (size_t)cnt;
+      key.poly[kKeyFileOrder[i]] = pk + off;
+      key.poly_len[kKeyFileOrder[i]] = (size_t)cnt;
       off += cnt * 32;
       if (!need(eval_size)) return fail(short_rc, "NotEnoughBytes: prover key evaluations");
       off += eval_size;  // recomputed on the device
@@ -943,7 +874,7 @@ int prover_from_bytes(const uint8_t* bytes, size_t len, const uint32_t* wires, s
   // VerifierKey::to_bytes (widget.rs:84-111)
   if (vk_len < 8 + 15 * 48) return fail(short_rc, "NotEnoughBytes: verifier key");
   if (le64(vk) != size) return fail(bad_rc, "InvalidData: verifier key domain differs from the prover's size");
-  for (int i = 0; i < N_POLY; i++) memcpy(key.comm[file_order[i]], vk + 8 + 48 * i, 48);
+  for (int i = 0; i < N_POLY; i++) memcpy(key.comm[kKeyFileOrder[i]], vk + 8 + 48 * i, 48);
   // CommitKey::from_raw_var_bytes: validated points
   size_t n_pts = 0;
   PB_TRY(raw_commit_key_parse(ck, ck_len, 1, &n_pts, nullptr));
@@ -969,17 +900,6 @@ void prover_free(pb200_prover* P) {
   delete P;
 }
 
-static pbh::Transcript base_transcript(const pb200_prover* P) {  // transcript.rs:131-145, widget.rs:218-257
-  pbh::Transcript tr(P->label.data(), P->label.size());
-  tr.circuit_domain_sep(P->constraints);
-  static const char* lbl[N_POLY] = {"q_m", "q_l", "q_r", "q_o", "q_c", "q_f", "q_arith", "q_range", "q_logic",
-                                    "q_variable_group_add", "q_fixed_group_add", "s_sigma_1", "s_sigma_2", "s_sigma_3", "s_sigma_4"};
-  static const int ord[N_POLY] = {Q_M, Q_L, Q_R, Q_O, Q_C, Q_F, Q_ARITH, Q_RANGE, Q_LOGIC, Q_VAR, Q_FIXED, S1, S2, S3, S4};
-  for (int i = 0; i < N_POLY; i++) tr.append_commitment(lbl[i], P->comm[ord[i]]);
-  tr.circuit_domain_sep(P->constraints);
-  return tr;
-}
-
 // Prover::prove_inner, V3.  d_wit: n_witnesses Fr on the device; pi_*: host.
 int prove_dev(const pb200_prover* P, const uint64_t* d_wit, const uint64_t* pi_idx, const uint64_t* pi_vals, size_t n_pi,
               const uint64_t* blinders_host, uint8_t* out_proof, cudaStream_t st) {
@@ -1000,7 +920,8 @@ int prove_dev(const pb200_prover* P, const uint64_t* d_wit, const uint64_t* pi_i
     return e ? atoi(e) : 2;
   }();
   const HFr* BL = (const HFr*)blinders_host;
-  pbh::Transcript tr = base_transcript(P);
+  // the prover's own constraint count stands for VerifierKey::n
+  pbh::Transcript tr = pbh::seed_transcript(P->label.data(), P->label.size(), P->constraints, P->comm[0], P->constraints);
   const HFr* PIV = (const HFr*)pi_vals;
   if (n_pi && (!pi_idx || !pi_vals)) return fail(PB200_ERR_INVALID_ARG, "public inputs announced but not given");
   for (size_t i = 0; i < n_pi; i++) {
@@ -1064,7 +985,8 @@ int prove_dev(const pb200_prover* P, const uint64_t* d_wit, const uint64_t* pi_i
   PB_ALLOC(scope, flag, 4);
 
   uint64_t aff[4 * 12];
-  uint8_t c48[11][48];
+  uint8_t c48[N_COMM][48];
+  Challenges ch;
 
   // ---- round 1 -------------------------------------------------------------------------------
   PB_LAUNCH(k_gather_wires, dim3(div_up(n, 256), 4), 256, 0, st, (const uint4*)d_wit, (const uint32_t*)P->d_wires, P->constraints, n, wv);
@@ -1103,16 +1025,11 @@ int prove_dev(const pb200_prover* P, const uint64_t* d_wit, const uint64_t* pi_i
     t_msm_throughput_hint = (hint_at > 0 && (g_force_throughput.load(std::memory_order_relaxed) || P->active.load(std::memory_order_relaxed) >= hint_at)) ? 1 : 0;
     PB_TRY(msm_run(P->srs, 0, (const uint64_t*)wp, n + 2, 4, stride, aff, st, ar));
   }
-  for (int k = 0; k < 4; k++) compress_affine(aff + 12 * k, c48[k]);
-  tr.append_commitment("a_comm", c48[0]);
-  tr.append_commitment("b_comm", c48[1]);
-  tr.append_commitment("c_comm", c48[2]);
-  tr.append_commitment("d_comm", c48[3]);
+  for (int k = 0; k < 4; k++) compress_affine(aff + 12 * k, c48[C_A + k]);
 
   // ---- round 2 -------------------------------------------------------------------------------
-  const HFr beta = tr.challenge_scalar("beta");
-  tr.append_scalar("beta", beta);
-  const HFr gamma = tr.challenge_scalar("gamma");
+  pbh::challenge_beta_gamma(tr, c48[0], ch);
+  const HFr beta = ch.beta, gamma = ch.gamma;
   PB_LAUNCH(k_perm_terms, div_up(n, 128), 128, 0, st, (const uint4*)wv, (const uint4*)P->d_sigma, w_half, n, to_dev(beta), to_dev(gamma), num, den);
   PB_LAUNCH(k_batch_div, div_up(div_up(n, 8), 128), 128, 0, st, (const uint4*)num, (const uint4*)den, n, num);
   PB_TRY((fr_scan<true, false>(num, n, den, st, ar)));  // den <- permutation vector z[i] = prod_{j<i} num_j/den_j
@@ -1126,15 +1043,11 @@ int prove_dev(const pb200_prover* P, const uint64_t* d_wit, const uint64_t* pi_i
   }
   t_msm_throughput_hint = (hint_at > 0 && (g_force_throughput.load(std::memory_order_relaxed) || P->active.load(std::memory_order_relaxed) >= hint_at)) ? 1 : 0;
   PB_TRY(msm_run(P->srs, 0, (const uint64_t*)zp, n + 3, 1, stride, aff, st, ar));
-  compress_affine(aff, c48[4]);
-  tr.append_commitment("z_comm", c48[4]);
+  compress_affine(aff, c48[C_Z]);
 
   // ---- round 3 -------------------------------------------------------------------------------
-  const HFr alpha = tr.challenge_scalar("alpha");
-  const HFr ch_range = tr.challenge_scalar("range separation challenge");
-  const HFr ch_logic = tr.challenge_scalar("logic separation challenge");
-  const HFr ch_fixed = tr.challenge_scalar("fixed base separation challenge");
-  const HFr ch_var = tr.challenge_scalar("variable base separation challenge");
+  pbh::challenge_alpha(tr, c48[0], ch);
+  const HFr alpha = ch.alpha;
   // t(X) has at most 4n + 7 coefficients, so the six coset transforms, the pointwise pass and the
   // inverse transform run on the 4n coset (the even points of the 8n one) and the top seven coefficients
   // are recovered from eight further points; the algebra is validated against the oracle in
@@ -1151,13 +1064,13 @@ int prove_dev(const pb200_prover* P, const uint64_t* d_wit, const uint64_t* pi_i
   {
     q.w8 = w8; q.key8 = P->d_key8; q.linear8 = P->d_linear8; q.l1_8 = P->d_l1_8; q.out = quot; q.n8 = n8;
     q.alpha = to_dev(alpha); q.beta = to_dev(beta); q.gamma = to_dev(gamma); q.alpha_sq = to_dev(alpha.sqr());
-    auto powers = [](const HFr& ch) {
-      const HFr k = ch.sqr(), k2 = k.sqr(), k3 = k2 * k;
-      WidgetCh w;
-      w.ch = to_dev(ch); w.k = to_dev(k); w.k2 = to_dev(k2); w.k3 = to_dev(k3); w.k4 = to_dev(k3 * k);
-      return w;
+    auto powers = [](const HFr& c) {
+      const SepPowers<HFr> h = sep_powers(c);
+      SepPowers<Fr> s;
+      s.ch = to_dev(h.ch); s.k = to_dev(h.k); s.k2 = to_dev(h.k2); s.k3 = to_dev(h.k3); s.k4 = to_dev(h.k4);
+      return s;
     };
-    q.ch_range = powers(ch_range); q.ch_logic = powers(ch_logic); q.ch_fixed = powers(ch_fixed); q.ch_var = powers(ch_var);
+    q.ch_range = powers(ch.range); q.ch_logic = powers(ch.logic); q.ch_fixed = powers(ch.fixed); q.ch_var = powers(ch.var);
     q.edwards_d = P->edwards_d;
     for (int i = 0; i < 8; i++) q.vh_inv[i] = to_dev(P->vh_inv[i]);
     q.has_range = P->has_widget[0]; q.has_logic = P->has_widget[1]; q.has_fixed = P->has_widget[2]; q.has_var = P->has_widget[3];
@@ -1238,17 +1151,13 @@ int prove_dev(const pb200_prover* P, const uint64_t* d_wit, const uint64_t* pi_i
   t_msm_throughput_hint = (hint_at > 0 && (g_force_throughput.load(std::memory_order_relaxed) || P->active.load(std::memory_order_relaxed) >= hint_at)) ? 1 : 0;
   PB_TRY(msm_run(P->srs, 0, (const uint64_t*)tq, tlen, 4, stride, aff, st, ar));  // synchronises the stream
   if (h_flag) return fail(PB200_ERR_UNSATISFIED, "CircuitUnsatisfied");
-  for (int k = 0; k < 4; k++) compress_affine(aff + 12 * k, c48[5 + k]);
-  tr.append_commitment("t_low_comm", c48[5]);
-  tr.append_commitment("t_mid_comm", c48[6]);
-  tr.append_commitment("t_high_comm", c48[7]);
-  tr.append_commitment("t_fourth_comm", c48[8]);
+  for (int k = 0; k < 4; k++) compress_affine(aff + 12 * k, c48[C_T_LOW + k]);
 
   // ---- round 4 -------------------------------------------------------------------------------
-  const HFr z_ch = tr.challenge_scalar("z_challenge");
+  pbh::challenge_z(tr, c48[0], ch);
+  const HFr z_ch = ch.z;
   const HFr zw = z_ch * to_host(ntt_group_gen(log_n, false));
-  enum { E_A, E_B, E_C, E_D, E_AW, E_BW, E_DW, E_QARITH, E_QC, E_QL, E_QR, E_S1, E_S2, E_S3, E_Z };
-  HFr ev[15];
+  HFr ev[N_EVAL];  // in Proof::to_bytes order
   {
     EvalJobs jobs;
     jobs.njobs = 15;
@@ -1272,88 +1181,32 @@ int prove_dev(const pb200_prover* P, const uint64_t* d_wit, const uint64_t* pi_i
     PB_CUDA(stream_wait(st));
     memcpy(ev, stage, 15 * 32);
   }
-  tr.append_scalar("a_eval", ev[E_A]); tr.append_scalar("b_eval", ev[E_B]); tr.append_scalar("c_eval", ev[E_C]); tr.append_scalar("d_eval", ev[E_D]);
-  tr.append_scalar("s_sigma_1_eval", ev[E_S1]); tr.append_scalar("s_sigma_2_eval", ev[E_S2]); tr.append_scalar("s_sigma_3_eval", ev[E_S3]);
-  tr.append_scalar("z_eval", ev[E_Z]);
-  tr.append_scalar("a_w_eval", ev[E_AW]); tr.append_scalar("b_w_eval", ev[E_BW]); tr.append_scalar("d_w_eval", ev[E_DW]);
-  tr.append_scalar("q_arith_eval", ev[E_QARITH]); tr.append_scalar("q_c_eval", ev[E_QC]); tr.append_scalar("q_l_eval", ev[E_QL]); tr.append_scalar("q_r_eval", ev[E_QR]);
-
   // ---- round 5 -------------------------------------------------------------------------------
-  const HFr v = tr.challenge_scalar("v_challenge");
-  const HFr v_w = tr.challenge_scalar("v_w_challenge");  // nothing is appended in between (prover.rs:680-730)
+  pbh::challenge_v(tr, ev, ch);
+  const HFr v = ch.v, v_w = ch.v_w;
   {
-    // host-side widget scalars of the linearisation polynomial (all widget compute_linearization)
-    auto h4 = [](const HFr& x) { return x.dbl().dbl(); };
-    auto delta = [](const HFr& f) { HFr o = HFr::one(); HFr f1 = f - o, f2 = f1 - o, f3 = f2 - o; return f * f1 * f2 * f3; };
-    auto small = [](uint64_t k) { return HFr::from_u64(k); };
-    const HFr &a = ev[E_A], &b = ev[E_B], &c = ev[E_C], &d = ev[E_D], &a_w = ev[E_AW], &b_w = ev[E_BW], &d_w = ev[E_DW];
-    HFr s_range, s_logic, s_fixed, s_var;
-    {
-      HFr k = ch_range.sqr(), k2 = k.sqr(), k3 = k2 * k;
-      s_range = (delta(c - h4(d)) + delta(b - h4(c)) * k + delta(a - h4(b)) * k2 + delta(d_w - h4(a)) * k3) * ch_range;
-    }
-    {
-      HFr k = ch_logic.sqr(), k2 = k.sqr(), k3 = k2 * k, k4 = k3 * k;
-      HFr A = a_w - h4(a), B = b_w - h4(b), D = d_w - h4(d);
-      const HFr& w = c;
-      HFr F = w * (w * (h4(w) - small(18) * (A + B) + small(81)) + small(18) * (A.sqr() + B.sqr()) - small(81) * (A + B) + small(83));
-      HFr E = small(3) * (A + B + D) - F.dbl();
-      HFr Bq = ev[E_QC] * (small(9) * D - small(3) * (A + B));
-      s_logic = (delta(A) + delta(B) * k + delta(D) * k2 + (w - A * B) * k3 + (Bq + E) * k4) * ch_logic;
-    }
-    const HFr ed = (small(10240) * small(10241).inv()).neg();
-    {
-      HFr one = HFr::one(), k = ch_fixed.sqr(), k2 = k.sqr(), k3 = k2 * k;
-      HFr bit = d_w - d - d;
-      HFr bit_c = bit * (bit - one) * (bit + one);
-      HFr y_alpha = bit.sqr() * (ev[E_QR] - one) + one, x_alpha = bit * ev[E_QL];
-      HFr xy = (bit * ev[E_QC] - c) * k;
-      HFr t = c * a * b * ed;
-      HFr xa = ((a_w + a_w * t) - (a * y_alpha + b * x_alpha)) * k2;
-      HFr ya = ((b_w - b_w * t) - (b * y_alpha + a * x_alpha)) * k3;
-      s_fixed = (bit_c + xa + ya + xy) * ch_fixed;
-    }
-    {
-      HFr k = ch_var.sqr();
-      HFr xy = a * d - d_w, y1x2 = b * c, y1y2 = b * d, x1x2 = a * c;
-      HFr t = ed * d_w * y1x2;
-      HFr x3c = ((d_w + y1x2) - (a_w + a_w * t)) * k;
-      HFr y3c = ((y1y2 + x1x2) - (b_w - b_w * t)) * k.sqr();
-      s_var = (xy + x3c + y3c) * ch_var;
-    }
-    const HFr bz = beta * z_ch;
-    const HFr s_ident = (a + bz + gamma) * (b + small(7) * bz + gamma) * (c + small(13) * bz + gamma) * (d + small(17) * bz + gamma) * alpha;
-    const HFr s_copy = (a + beta * ev[E_S1] + gamma) * (b + beta * ev[E_S2] + gamma) * (c + beta * ev[E_S3] + gamma) * (beta * ev[E_Z]) * alpha;
-    const HFr z_n = hfr_pow(z_ch, n);
+    const HFr z_n = z_ch.pow_u64(n);
     // domain of z_poly.degree() - 2 is the proving domain n (permutation/proverkey.rs:156-163)
     const HFr l1_z = (z_n - HFr::one()) * to_host(ntt_size_inv(log_n)) * (z_ch - HFr::one()).inv();
-    const HFr zh = (z_n - HFr::one()).neg();
+    const LinScalars ls = linearisation_scalars(ev, ch, z_n, l1_z);
     HFr vp[12];
     vp[0] = HFr::one();
     for (int i = 1; i < 12; i++) vp[i] = vp[i - 1] * v;
+    HFr sel[N_POLY];
+    for (int k = 0; k < N_POLY; k++) sel[k] = ls.sel[k];
+    sel[Q_ARITH] = sel[Q_ARITH] + vp[8];
+    sel[Q_C] = sel[Q_C] + vp[9];
+    sel[Q_L] = sel[Q_L] + vp[10];
+    sel[Q_R] = sel[Q_R] + vp[11];
     auto poly = [&](int k) { return (const uint4*)(P->d_polys + 2 * (size_t)k * n); };
-    const HFr qa = ev[E_QARITH];
     // W_z numerator: r + v a + v^2 b + v^3 c + v^4 d + v^5 s1 + v^6 s2 + v^7 s3 + v^8 q_arith + v^9 q_c + v^10 q_l + v^11 q_r
     LinArgs la;
     int t = 0;
     auto term = [&](const uint4* p, size_t len, const HFr& coef) { la.poly[t] = p; la.len[t] = (unsigned)len; la.coef[t] = to_dev(coef); t++; };
-    term(poly(Q_M), n, a * b * qa);
-    term(poly(Q_L), n, a * qa + vp[10]);
-    term(poly(Q_R), n, b * qa + vp[11]);
-    term(poly(Q_O), n, c * qa);
-    term(poly(Q_F), n, d * qa);
-    term(poly(Q_C), n, qa + vp[9]);
-    term(poly(Q_ARITH), n, vp[8]);
-    term(poly(Q_RANGE), n, s_range);
-    term(poly(Q_LOGIC), n, s_logic);
-    term(poly(Q_FIXED), n, s_fixed);
-    term(poly(Q_VAR), n, s_var);
-    term(zp, n + 3, s_ident + l1_z * alpha.sqr());
-    term(poly(S4), n, s_copy.neg());
-    term(tq, stride, zh);
-    term(tq + 2 * stride, stride, zh * z_n);
-    term(tq + 4 * stride, stride, zh * z_n.sqr());
-    term(tq + 6 * stride, stride, zh * z_n.sqr() * z_n);
+    for (int k = Q_M; k <= Q_VAR; k++) term(poly(k), n, sel[k]);
+    term(zp, n + 3, ls.z);
+    term(poly(S4), n, sel[S4]);
+    for (int j = 0; j < 4; j++) term(tq + 2 * j * stride, stride, ls.t[j]);
     term(wp, n + 2, vp[1]);
     term(wp + 2 * stride, n + 2, vp[2]);
     term(wp + 4 * stride, n + 2, vp[3]);
@@ -1389,14 +1242,14 @@ int prove_dev(const pb200_prover* P, const uint64_t* d_wit, const uint64_t* pi_i
     const size_t wlen = std::min(stride, key_len);
     t_msm_throughput_hint = (hint_at > 0 && (g_force_throughput.load(std::memory_order_relaxed) || P->active.load(std::memory_order_relaxed) >= hint_at)) ? 1 : 0;
     PB_TRY(msm_run(P->srs, 0, (const uint64_t*)agg, wlen, 2, stride, aff, st, ar));
-    compress_affine(aff, c48[9]);
-    compress_affine(aff + 12, c48[10]);
+    compress_affine(aff, c48[C_W_Z]);
+    compress_affine(aff + 12, c48[C_W_ZW]);
   }
   // Proof::to_bytes (proof.rs:137-162, linearization_poly.rs:98-124)
-  for (int i = 0; i < 11; i++) memcpy(out_proof + 48 * i, c48[i], 48);
-  for (int i = 0; i < 15; i++) {
+  memcpy(out_proof, c48, sizeof c48);
+  for (int i = 0; i < N_EVAL; i++) {
     HFr cnon = ev[i].from_mont();
-    memcpy(out_proof + 528 + 32 * i, cnon.v, 32);
+    memcpy(out_proof + kProofEvalAt + 32 * i, cnon.v, 32);
   }
   return 0;
 }

@@ -6,6 +6,7 @@
 #include <string.h>
 
 #include "host_field.h"
+#include "plonk_algebra.cuh"
 
 namespace pbh {
 
@@ -134,5 +135,67 @@ class Transcript {
  private:
   Strobe128 s_;
 };
+
+// ---- The V3 schedule: what goes into the transcript, in which order, under which label ----------------------
+// Prover::prove_inner (prover.rs:415-761) and Proof::verify (proof.rs:218-300) run the same sequence.  The
+// commitments are read from `comms`, the 11 compressed commitments in Proof::to_bytes order.
+
+// Transcript::base (transcript.rs:131-145) with VerifierKey::seed_transcript (widget.rs:218-257).  key_comms: the 15
+// key commitments in pb::Poly order; vk_n: VerifierKey::n, which seed_transcript_inner appends last.
+inline Transcript seed_transcript(const uint8_t* label, size_t label_len, uint64_t constraints, const uint8_t* key_comms, uint64_t vk_n) {
+  Transcript tr(label, label_len);
+  tr.circuit_domain_sep(constraints);
+  for (const pb::SeedEntry& s : pb::kSeedOrder) tr.append_commitment(s.label, key_comms + 48 * s.poly);
+  tr.circuit_domain_sep(vk_n);
+  return tr;
+}
+// The wire commitments -> beta, gamma.
+inline void challenge_beta_gamma(Transcript& tr, const uint8_t* comms, pb::Challenges& c) {
+  tr.append_commitment("a_comm", comms + 48 * pb::C_A);
+  tr.append_commitment("b_comm", comms + 48 * pb::C_B);
+  tr.append_commitment("c_comm", comms + 48 * pb::C_C);
+  tr.append_commitment("d_comm", comms + 48 * pb::C_D);
+  c.beta = tr.challenge_scalar("beta");
+  tr.append_scalar("beta", c.beta);
+  c.gamma = tr.challenge_scalar("gamma");
+}
+// The permutation commitment -> alpha and the four separation challenges.
+inline void challenge_alpha(Transcript& tr, const uint8_t* comms, pb::Challenges& c) {
+  tr.append_commitment("z_comm", comms + 48 * pb::C_Z);
+  c.alpha = tr.challenge_scalar("alpha");
+  c.range = tr.challenge_scalar("range separation challenge");
+  c.logic = tr.challenge_scalar("logic separation challenge");
+  c.fixed = tr.challenge_scalar("fixed base separation challenge");
+  c.var = tr.challenge_scalar("variable base separation challenge");
+}
+// The quotient commitments -> the evaluation point z.
+inline void challenge_z(Transcript& tr, const uint8_t* comms, pb::Challenges& c) {
+  tr.append_commitment("t_low_comm", comms + 48 * pb::C_T_LOW);
+  tr.append_commitment("t_mid_comm", comms + 48 * pb::C_T_MID);
+  tr.append_commitment("t_high_comm", comms + 48 * pb::C_T_HIGH);
+  tr.append_commitment("t_fourth_comm", comms + 48 * pb::C_T_FOURTH);
+  c.z = tr.challenge_scalar("z_challenge");
+}
+// The 15 evaluations (pb::ProofEval order, Montgomery form) -> v, v_w.  They are appended in an order of their own;
+// nothing is appended between the two challenges (prover.rs:680-730).
+inline void challenge_v(Transcript& tr, const HFr ev[pb::N_EVAL], pb::Challenges& c) {
+  static const struct {
+    const char* label;
+    int eval;
+  } order[pb::N_EVAL] = {{"a_eval", pb::E_A},         {"b_eval", pb::E_B},         {"c_eval", pb::E_C},
+                         {"d_eval", pb::E_D},         {"s_sigma_1_eval", pb::E_S1}, {"s_sigma_2_eval", pb::E_S2},
+                         {"s_sigma_3_eval", pb::E_S3}, {"z_eval", pb::E_Z},          {"a_w_eval", pb::E_AW},
+                         {"b_w_eval", pb::E_BW},       {"d_w_eval", pb::E_DW},       {"q_arith_eval", pb::E_QARITH},
+                         {"q_c_eval", pb::E_QC},       {"q_l_eval", pb::E_QL},       {"q_r_eval", pb::E_QR}};
+  for (const auto& o : order) tr.append_scalar(o.label, ev[o.eval]);
+  c.v = tr.challenge_scalar("v_challenge");
+  c.v_w = tr.challenge_scalar("v_w_challenge");
+}
+// The two opening commitments -> u (the Verifier's batching challenge; the prover stops before it).
+inline void challenge_u(Transcript& tr, const uint8_t* comms, pb::Challenges& c) {
+  tr.append_commitment("w_z_chall_comm", comms + 48 * pb::C_W_Z);
+  tr.append_commitment("w_z_chall_w_comm", comms + 48 * pb::C_W_ZW);
+  c.u = tr.challenge_scalar("u_challenge");
+}
 
 }  // namespace pbh

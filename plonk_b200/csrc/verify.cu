@@ -14,13 +14,14 @@
 #include "g1.cuh"
 #include "host_field.h"
 #include "pairing.cuh"
+#include "plonk_algebra.cuh"
 #include "transcript.h"
 
 struct pb200_verifier {
   std::vector<uint8_t> label;
   uint64_t vk_n = 0;                          // VerifierKey::n: the constraint count for a compiled circuit
   uint64_t n = 0, size = 0, constraints = 0;  // the domain size (EvaluationDomain::new(vk_n)), Verifier::size, Verifier::constraints
-  uint8_t vk_comm[15][48];                     // pb200_prover_commitments order
+  uint8_t vk_comm[pb::N_POLY][48];             // pb::Poly order
   uint8_t opening_key[PB200_OPENING_KEY_BYTES];
   std::vector<uint64_t> pi_idx;
   std::vector<pbh::HFr> pi_roots;  // group_gen_inv^index
@@ -216,54 +217,25 @@ bool fr_canonical(const uint8_t* b, HFr* out) {  // BlsScalar::from_bytes: littl
   *out = out->to_mont();
   return true;
 }
-HFr fr_pow(HFr b, uint64_t e) {
-  HFr r = HFr::one();
-  for (; e; e >>= 1, b = b.sqr())
-    if (e & 1) r = r * b;
-  return r;
-}
 
 // Proof::verify up to the pairing: the transcript replay and the 32 scalars of k_verify_msm (canonical form).
 // Returns PB200_OK, PB200_ERR_POINT_MALFORMED for a non-canonical evaluation or PB200_ERR_VERIFY.
 int verify_scalars(const pb200_verifier* V, const uint8_t* proof, const HFr* pi, uint64_t* out) {
-  enum { A, B, C, D, AW, BW, DW, QARITH, QC, QL, QR, S1, S2, S3, Z };
-  HFr e[15];
-  for (int k = 0; k < 15; k++)
-    if (!fr_canonical(proof + 528 + 32 * k, &e[k])) return PB200_ERR_POINT_MALFORMED;
-  const uint8_t* cm = proof;  // a, b, c, d, z, t_low, t_mid, t_high, t_fourth, w_z, w_zw
+  HFr e[N_EVAL];
+  for (int k = 0; k < N_EVAL; k++)
+    if (!fr_canonical(proof + kProofEvalAt + 32 * k, &e[k])) return PB200_ERR_POINT_MALFORMED;
   pbh::Transcript tr = V->base;
   for (size_t k = 0; k < V->pi_idx.size(); k++) tr.append_scalar("pi", pi[k]);
-  tr.append_commitment("a_comm", cm + 0);
-  tr.append_commitment("b_comm", cm + 48);
-  tr.append_commitment("c_comm", cm + 96);
-  tr.append_commitment("d_comm", cm + 144);
-  const HFr beta = tr.challenge_scalar("beta");
-  tr.append_scalar("beta", beta);
-  const HFr gamma = tr.challenge_scalar("gamma");
-  tr.append_commitment("z_comm", cm + 192);
-  const HFr alpha = tr.challenge_scalar("alpha");
-  const HFr ch_range = tr.challenge_scalar("range separation challenge");
-  const HFr ch_logic = tr.challenge_scalar("logic separation challenge");
-  const HFr ch_fixed = tr.challenge_scalar("fixed base separation challenge");
-  const HFr ch_var = tr.challenge_scalar("variable base separation challenge");
-  tr.append_commitment("t_low_comm", cm + 240);
-  tr.append_commitment("t_mid_comm", cm + 288);
-  tr.append_commitment("t_high_comm", cm + 336);
-  tr.append_commitment("t_fourth_comm", cm + 384);
-  const HFr z = tr.challenge_scalar("z_challenge");
-  tr.append_scalar("a_eval", e[A]); tr.append_scalar("b_eval", e[B]); tr.append_scalar("c_eval", e[C]); tr.append_scalar("d_eval", e[D]);
-  tr.append_scalar("s_sigma_1_eval", e[S1]); tr.append_scalar("s_sigma_2_eval", e[S2]); tr.append_scalar("s_sigma_3_eval", e[S3]);
-  tr.append_scalar("z_eval", e[Z]);
-  tr.append_scalar("a_w_eval", e[AW]); tr.append_scalar("b_w_eval", e[BW]); tr.append_scalar("d_w_eval", e[DW]);
-  tr.append_scalar("q_arith_eval", e[QARITH]); tr.append_scalar("q_c_eval", e[QC]); tr.append_scalar("q_l_eval", e[QL]); tr.append_scalar("q_r_eval", e[QR]);
-  const HFr v = tr.challenge_scalar("v_challenge");
-  const HFr v_w = tr.challenge_scalar("v_w_challenge");
-  tr.append_commitment("w_z_chall_comm", cm + 432);
-  tr.append_commitment("w_z_chall_w_comm", cm + 480);
-  const HFr u = tr.challenge_scalar("u_challenge");
+  Challenges c;
+  pbh::challenge_beta_gamma(tr, proof, c);
+  pbh::challenge_alpha(tr, proof, c);
+  pbh::challenge_z(tr, proof, c);
+  pbh::challenge_v(tr, e, c);
+  pbh::challenge_u(tr, proof, c);
+  const HFr &z = c.z, &v = c.v, &v_w = c.v_w, &u = c.u;
 
   const HFr one = HFr::one();
-  const HFr z_n = fr_pow(z, V->n), z_h = z_n - one;
+  const HFr z_n = z.pow_u64(V->n), z_h = z_n - one;
   // compute_lagrange_and_barycentric_evaluations (proof.rs:997-1040): one batch inversion
   std::vector<HFr> den, pref;
   std::vector<size_t> which;
@@ -291,71 +263,27 @@ int verify_scalars(const pb200_verifier* V, const uint8_t* proof, const HFr* pi,
   for (size_t j = 0; j < which.size(); j++) pi_eval = pi_eval + den[1 + j] * pi[which[j]];
   pi_eval = pi_eval * z_h * V->size_inv;
 
-  const HFr alpha_sq = alpha.sqr();
-  const HFr perm = (e[A] + beta * e[S1] + gamma) * (e[B] + beta * e[S2] + gamma) * (e[C] + beta * e[S3] + gamma);
-  const HFr r0 = pi_eval - l1 * alpha_sq - alpha * perm * (e[D] + gamma) * e[Z];
+  const HFr perm = perm_copy3(eval_wires(e), c.beta, c.gamma, [&](int j) { return e[E_S1 + j]; });
+  const HFr r0 = pi_eval - l1 * c.alpha.sqr() - c.alpha * perm * (e[E_D] + c.gamma) * e[E_Z];
   HFr vc[14];
   vc[0] = v;
   for (int k = 1; k < 11; k++) vc[k] = vc[k - 1] * v;
   vc[11] = v_w * u;
   vc[12] = vc[11] * v_w;
   vc[13] = vc[12] * v_w;
-  const int eo[14] = {A, B, C, D, S1, S2, S3, QARITH, QC, QL, QR, AW, BW, DW};
-  HFr E = u * e[Z] - r0;
+  const int eo[14] = {E_A, E_B, E_C, E_D, E_S1, E_S2, E_S3, E_QARITH, E_QC, E_QL, E_QR, E_AW, E_BW, E_DW};
+  HFr E = u * e[E_Z] - r0;
   for (int k = 0; k < 14; k++) E = E + e[eo[k]] * vc[k];
 
-  // widget scalars (range, logic, fixed_base, curve_addition verifierkey.rs)
-  auto h4 = [](const HFr& x) { return x.dbl().dbl(); };
-  auto delta = [&](const HFr& f) { const HFr f1 = f - one, f2 = f1 - one, f3 = f2 - one; return f * f1 * f2 * f3; };
-  auto small = [](uint64_t k) { return HFr::from_u64(k); };
-  const HFr &a = e[A], &b = e[B], &c = e[C], &d = e[D], &a_w = e[AW], &b_w = e[BW], &d_w = e[DW];
-  HFr s_range, s_logic, s_fixed, s_var;
-  {
-    const HFr k = ch_range.sqr(), k2 = k.sqr(), k3 = k2 * k;
-    s_range = (delta(c - h4(d)) + delta(b - h4(c)) * k + delta(a - h4(b)) * k2 + delta(d_w - h4(a)) * k3) * ch_range;
-  }
-  {
-    const HFr k = ch_logic.sqr(), k2 = k.sqr(), k3 = k2 * k, k4 = k3 * k;
-    const HFr Aa = a_w - h4(a), Bb = b_w - h4(b), Dd = d_w - h4(d);
-    const HFr& w = c;
-    const HFr F = w * (w * (h4(w) - small(18) * (Aa + Bb) + small(81)) + small(18) * (Aa.sqr() + Bb.sqr()) - small(81) * (Aa + Bb) + small(83));
-    const HFr Ee = small(3) * (Aa + Bb + Dd) - F.dbl();
-    const HFr Bq = e[QC] * (small(9) * Dd - small(3) * (Aa + Bb));
-    s_logic = (delta(Aa) + delta(Bb) * k + delta(Dd) * k2 + (w - Aa * Bb) * k3 + (Bq + Ee) * k4) * ch_logic;
-  }
-  const HFr ed = (small(10240) * small(10241).inv()).neg();
-  {
-    const HFr k = ch_fixed.sqr(), k2 = k.sqr(), k3 = k2 * k;
-    const HFr bit = d_w - d - d;
-    const HFr bit_c = bit * (bit - one) * (bit + one);
-    const HFr y_alpha = bit.sqr() * (e[QR] - one) + one, x_alpha = bit * e[QL];
-    const HFr xy = (bit * e[QC] - c) * k;
-    const HFr t = c * a * b * ed;
-    const HFr xa = ((a_w + a_w * t) - (a * y_alpha + b * x_alpha)) * k2;
-    const HFr ya = ((b_w - b_w * t) - (b * y_alpha + a * x_alpha)) * k3;
-    s_fixed = (bit_c + xa + ya + xy) * ch_fixed;
-  }
-  {
-    const HFr k = ch_var.sqr();
-    const HFr xy = a * d - d_w, y1x2 = b * c, y1y2 = b * d, x1x2 = a * c;
-    const HFr t = ed * d_w * y1x2;
-    const HFr x3c = ((d_w + y1x2) - (a_w + a_w * t)) * k;
-    const HFr y3c = ((y1y2 + x1x2) - (b_w - b_w * t)) * k.sqr();
-    s_var = (xy + x3c + y3c) * ch_var;
-  }
-  // permutation verifierkey.rs
-  const HFr bz = beta * z;
-  const HFr xs = (a + bz + gamma) * (b + small(7) * bz + gamma) * (c + small(13) * bz + gamma) * (d + small(17) * bz + gamma) * alpha;
-  const HFr ys = perm * (beta * e[Z]) * alpha;
+  const LinScalars ls = linearisation_scalars(e, c, z_n, l1);
   HFr f[11];
   for (int k = 0; k < 11; k++) f[k] = vc[k];
   f[0] = f[0] + vc[11];
   f[1] = f[1] + vc[12];
   f[3] = f[3] + vc[13];
-  const HFr qa = e[QARITH];
-  const HFr s[PB_VERIFY_TERMS] = {a * b * qa, a * qa, b * qa, c * qa, d * qa, qa, s_range, s_logic, s_fixed, s_var,
-                                  xs + l1 * alpha_sq + u, ys.neg(), z_h.neg(), z_n * z_h.neg(), z_n.sqr() * z_h.neg(),
-                                  z_n.sqr() * z_n * z_h.neg(), f[0], f[1], f[2], f[3], f[4], f[5], f[6], f[7], f[8], f[9], f[10],
+  const HFr s[PB_VERIFY_TERMS] = {ls.sel[Q_M], ls.sel[Q_L], ls.sel[Q_R], ls.sel[Q_O], ls.sel[Q_F], ls.sel[Q_C], ls.sel[Q_RANGE],
+                                  ls.sel[Q_LOGIC], ls.sel[Q_FIXED], ls.sel[Q_VAR], ls.z + u, ls.sel[S4], ls.t[0], ls.t[1], ls.t[2],
+                                  ls.t[3], f[0], f[1], f[2], f[3], f[4], f[5], f[6], f[7], f[8], f[9], f[10],
                                   E.neg(), z, u * z * V->group_gen, HFr::zero(), u};
   for (int k = 0; k < PB_VERIFY_TERMS; k++) {
     const HFr cn = s[k].from_mont();
@@ -373,9 +301,7 @@ void put_be64(std::vector<uint8_t>& o, uint64_t x) {
   for (int k = 7; k >= 0; k--) o.push_back((uint8_t)(x >> (8 * k)));
 }
 
-// VerifierKey::to_bytes (widget.rs:84-111) orders the commitments q_m, q_l, q_r, q_o, q_f, q_c, q_arith, q_logic,
-// q_range, q_fixed_group_add, q_variable_group_add, s_sigma_1..4; pb200_prover_commitments has q_range before q_logic.
-const int kFileOrder[15] = {0, 1, 2, 3, 4, 5, 6, 8, 7, 9, 10, 11, 12, 13, 14};
+// VerifierKey::to_bytes (widget.rs:84-111): VerifierKey::n, the 15 commitments in kKeyFileOrder, then 5 more
 constexpr size_t kVerifierKeyBytes = 20 * 48 + 8;
 
 // Verifier::new (verifier.rs:32-60) from validated parts.  vk_n is VerifierKey::n, which Compiler::compile sets to the
@@ -429,15 +355,8 @@ int verifier_build(const uint8_t* label, size_t label_len, uint64_t vk_n, uint64
   V->size_fr = HFr::from_u64(V->n);
   V->size_inv = V->size_fr.inv();
   const HFr g_inv = g.inv();
-  for (uint64_t idx : V->pi_idx) V->pi_roots.push_back(fr_pow(g_inv, idx));
-  // Transcript::base (transcript.rs:131-145) with VerifierKey::seed_transcript (widget.rs:218-257)
-  V->base = pbh::Transcript(V->label.data(), V->label.size());
-  V->base.circuit_domain_sep(constraints);
-  static const char* lbl[15] = {"q_m", "q_l", "q_r", "q_o", "q_c", "q_f", "q_arith", "q_range", "q_logic",
-                                "q_variable_group_add", "q_fixed_group_add", "s_sigma_1", "s_sigma_2", "s_sigma_3", "s_sigma_4"};
-  static const int ord[15] = {0, 1, 2, 3, 5, 4, 6, 7, 8, 10, 9, 11, 12, 13, 14};
-  for (int k = 0; k < 15; k++) V->base.append_commitment(lbl[k], comms + 48 * ord[k]);
-  V->base.circuit_domain_sep(vk_n);  // seed_transcript_inner ends with VerifierKey::n (widget.rs:256)
+  for (uint64_t idx : V->pi_idx) V->pi_roots.push_back(g_inv.pow_u64(idx));
+  V->base = pbh::seed_transcript(V->label.data(), V->label.size(), constraints, comms, vk_n);
   cudaError_t e = cudaMalloc((void**)&V->d_points, 16 * 96);
   if (e == cudaSuccess) e = cudaMemcpy(V->d_points, raw.data(), 16 * 96, cudaMemcpyHostToDevice);
   if (e != cudaSuccess) {
@@ -491,7 +410,7 @@ int pb200_verifier_from_bytes(const uint8_t* bytes, size_t len, pb200_verifier_t
   uint8_t comms[15 * 48];
   for (int k = 0; k < 15; k++) memcpy(comms + 48 * k, vk + 8 + 48 * k, 48);
   uint8_t ordered[15 * 48];
-  for (int k = 0; k < 15; k++) memcpy(ordered + 48 * kFileOrder[k], comms + 48 * k, 48);
+  for (int k = 0; k < 15; k++) memcpy(ordered + 48 * kKeyFileOrder[k], comms + 48 * k, 48);
   std::vector<uint64_t> idx(n_pi);
   for (uint64_t k = 0; k < n_pi; k++) idx[k] = be64(pis + 8 * k);
   return verifier_build(label, label_len, n, size, constraints, ordered, okey, idx.data(), idx.size(), out);
@@ -509,7 +428,7 @@ int pb200_verifier_to_bytes(const pb200_verifier_t* V, uint8_t* out, size_t cap,
   o.insert(o.end(), V->label.begin(), V->label.end());
   const size_t vk_at = o.size();
   for (int k = 0; k < 8; k++) o.push_back((uint8_t)(V->vk_n >> (8 * k)));
-  for (int k = 0; k < 15; k++) o.insert(o.end(), V->vk_comm[kFileOrder[k]], V->vk_comm[kFileOrder[k]] + 48);
+  for (int k = 0; k < 15; k++) o.insert(o.end(), V->vk_comm[kKeyFileOrder[k]], V->vk_comm[kKeyFileOrder[k]] + 48);
   o.resize(vk_at + kVerifierKeyBytes, 0);
   o.insert(o.end(), V->opening_key, V->opening_key + PB200_OPENING_KEY_BYTES);
   for (uint64_t i : V->pi_idx) put_be64(o, i);
@@ -538,11 +457,11 @@ int pb200_verify(const pb200_verifier_t* V, const uint8_t* proofs, size_t n_proo
   // host: transcripts and scalars, spread over threads for large batches
   std::vector<uint64_t> scal(n_proofs * PB_VERIFY_TERMS * 4);
   std::vector<int> hstat(n_proofs);
-  std::vector<uint8_t> comm(n_proofs * 528);
+  std::vector<uint8_t> comm(n_proofs * kProofEvalAt);
   auto work = [&](size_t lo, size_t hi) {
     for (size_t i = lo; i < hi; i++) {
-      const uint8_t* pr = proofs + 1008 * i;
-      memcpy(comm.data() + 528 * i, pr, 528);
+      const uint8_t* pr = proofs + kProofBytes * i;
+      memcpy(comm.data() + kProofEvalAt * i, pr, kProofEvalAt);
       hstat[i] = verify_scalars(V, pr, (const HFr*)(pi_vals + 4 * n_pi * i), scal.data() + (size_t)PB_VERIFY_TERMS * 4 * i);
     }
   };
@@ -562,13 +481,13 @@ int pb200_verify(const pb200_verifier_t* V, const uint8_t* proofs, size_t n_proo
   uint4 *d_pts, *d_scal, *d_g1;
   unsigned* d_bad;
   int* d_stat;
-  PB_ALLOC(scope, d_comm, n_proofs * 528);
+  PB_ALLOC(scope, d_comm, n_proofs * kProofEvalAt);
   PB_ALLOC(scope, d_pts, n_proofs * 11 * 96);
   PB_ALLOC(scope, d_scal, scal.size() * 8);
   PB_ALLOC(scope, d_g1, n_proofs * 2 * 96);
   PB_ALLOC(scope, d_bad, 4);
   PB_ALLOC(scope, d_stat, n_proofs * sizeof(int));
-  PB_CUDA(cudaMemcpyAsync(d_comm, comm.data(), n_proofs * 528, cudaMemcpyHostToDevice, st));
+  PB_CUDA(cudaMemcpyAsync(d_comm, comm.data(), n_proofs * kProofEvalAt, cudaMemcpyHostToDevice, st));
   PB_CUDA(cudaMemcpyAsync(d_scal, scal.data(), scal.size() * 8, cudaMemcpyHostToDevice, st));
   PB_CUDA(cudaMemcpyAsync(d_stat, hstat.data(), n_proofs * sizeof(int), cudaMemcpyHostToDevice, st));
   g1_decompress_dev(d_comm, n_proofs * 11, d_pts, d_bad, st);
