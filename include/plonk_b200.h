@@ -14,6 +14,11 @@
  *                                    src/commitment_scheme/kzg10/commitment.rs:95-101
  *   pb200_prover_* / pb200_prove     Prover::new / Prover::prove (PlonkVersion::V3)
  *                                    src/compiler/prover.rs:53-115, 415-761
+ *   pb200_prove_with_version         Prover::prove_with_version (V2 and V3; V1 is refused as the reference does)
+ *                                    src/compiler/prover.rs:364-413
+ *   pb200_verifier_* / pb200_verify  Verifier / Verifier::verify (PlonkVersion::V3)
+ *   pb200_verify_with_version        Verifier::verify_with_version (V1, V2 and V3)
+ *                                    src/compiler/verifier.rs:32-263
  *
  * Data layout (identical to the reference's in-memory layout, SURVEY.md section 8):
  *   Fr  (BlsScalar)  4 x u64 little-endian limbs, Montgomery form R = 2^256        -> 32 bytes
@@ -49,8 +54,16 @@ typedef enum {
   /* -7 .. -9: circuit front end, plonk_b200_composer.h */
   PB200_ERR_POINT_MALFORMED = -10,/* dusk_bytes::Error::InvalidData / Error::PointMalformed: a G1 encoding that is
                                      not canonical, not on the curve or not in the prime-order subgroup */
-  PB200_ERR_VERIFY = -11          /* Error::ProofVerificationError: the proof does not satisfy the verifier */
+  PB200_ERR_VERIFY = -11,         /* Error::ProofVerificationError: the proof does not satisfy the verifier */
+  PB200_ERR_UNSUPPORTED_VERSION = -12 /* Error::UnsupportedProvingVersion: PlonkVersion::V1 proofs cannot be made */
 } pb200_status;
+
+/* PlonkVersion (src/compiler.rs:22-42), for the *_with_version calls.  V3 is the current profile and the one the
+ * calls without a version use.  V2 is the legacy transcript seed (Transcript::base: the commitment of s_sigma_1 goes
+ * in under the "s_sigma_4" label) with V3's opening checks.  V1 is the legacy seed with the legacy opening
+ * (Proof::verify_legacy, proof.rs:518-790), which does not bind the evaluations of q_arith, q_c, q_l and q_r: a V1
+ * verdict is meaningful only for proofs made under the old rules, as in the reference. */
+typedef enum { PB200_PLONK_V1 = 1, PB200_PLONK_V2 = 2, PB200_PLONK_V3 = 3 } pb200_plonk_version;
 
 typedef struct pb200_srs pb200_srs_t;
 typedef struct pb200_prover pb200_prover_t;
@@ -213,8 +226,18 @@ int pb200_prove(const pb200_prover_t* prover, const uint64_t* witnesses, size_t 
 int pb200_prove_dev(const pb200_prover_t* prover, const uint64_t* d_witnesses, size_t n_witnesses,
                     const uint64_t* pi_idx, const uint64_t* pi_vals, size_t n_pi,
                     const uint64_t* blinders, uint8_t* out_proof, void* stream);
+/* Prover::prove_with_version (prover.rs:364-413): pb200_prove / pb200_prove_dev under a pb200_plonk_version.
+ * PB200_PLONK_V3 is pb200_prove.  PB200_PLONK_V2 differs from it only in the transcript seed (Transcript::base);
+ * the library always supports it, as the reference does with its `legacy-proving` feature on.  PB200_PLONK_V1
+ * returns PB200_ERR_UNSUPPORTED_VERSION, any other value PB200_ERR_INVALID_ARG; neither touches the device. */
+int pb200_prove_with_version(const pb200_prover_t* prover, int version, const uint64_t* witnesses, size_t n_witnesses,
+                             const uint64_t* pi_idx, const uint64_t* pi_vals, size_t n_pi,
+                             const uint64_t* blinders, uint8_t* out_proof);
+int pb200_prove_dev_with_version(const pb200_prover_t* prover, int version, const uint64_t* d_witnesses, size_t n_witnesses,
+                                 const uint64_t* pi_idx, const uint64_t* pi_vals, size_t n_pi,
+                                 const uint64_t* blinders, uint8_t* out_proof, void* stream);
 
-/* ---- verifier (Verifier::verify, PlonkVersion::V3; src/compiler/verifier.rs) ---------------------------------- */
+/* ---- verifier (Verifier::verify and verify_with_version; src/compiler/verifier.rs) ----------------------------- */
 /* Compiler::compile's Verifier half: the label, the circuit's constraint count, the 15 verifier-key commitments in
  * pb200_prover_commitments order, OpeningKey::to_bytes (PB200_OPENING_KEY_BYTES: g compressed, then h and [x]h as
  * 96-byte compressed G2 points - zcash encoding, x.c1 then x.c0 big-endian) and the public-input positions.
@@ -239,9 +262,16 @@ void pb200_verifier_free(pb200_verifier_t* verifier);
  * pairing check fails, or z lies in the domain) or PB200_ERR_POINT_MALFORMED (Proof::from_bytes would fail: a
  * commitment that is not canonical, not on the curve or not torsion free, or a non-canonical evaluation).  A verdict
  * does not depend on the batch.  The call itself fails with PB200_ERR_INVALID_ARG when n_pi differs from the
- * verifier's public-input count (InconsistentPublicInputsLen). */
+ * verifier's public-input count (InconsistentPublicInputsLen).  pb200_verify checks PlonkVersion::V3. */
 int pb200_verify(const pb200_verifier_t* verifier, const uint8_t* proofs, size_t n_proofs, const uint64_t* pi_vals,
                  size_t n_pi, int32_t* status);
+/* Verifier::verify_with_version (verifier.rs:214-263): pb200_verify under a pb200_plonk_version, one version for the
+ * whole batch.  Same statuses and argument checks; an unknown version is PB200_ERR_INVALID_ARG.  PB200_PLONK_V3
+ * returns exactly what pb200_verify returns.  Every verifier, from pb200_verifier_new or _from_bytes, holds both
+ * base transcripts, so it accepts every version.  V1 does not bind the selector evaluations (see
+ * pb200_plonk_version); the device work per proof is the same for all three versions. */
+int pb200_verify_with_version(const pb200_verifier_t* verifier, int version, const uint8_t* proofs, size_t n_proofs,
+                              const uint64_t* pi_vals, size_t n_pi, int32_t* status);
 /* Tests only: the device pairing e(P_k, Q_k) for n G1 points (96-byte raw layout) and n compressed G2 points, as
  * Fp12 values of 576 bytes (c0.c0.c0, c0.c0.c1, c0.c1.c0, ..., c1.c2.c1; each Fp 6 x u64 Montgomery limbs). */
 int pb200_selftest_pairing(const uint64_t* g1_raw, const uint8_t* g2_compressed, size_t n, uint64_t* out_fp12);

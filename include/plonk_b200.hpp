@@ -6,8 +6,10 @@
 //   plonk_b200::EvaluationDomain   src/fft/domain.rs:35-232      new / fft / ifft / coset_fft / coset_ifft
 //   plonk_b200::CommitKey          src/commitment_scheme/kzg10/key.rs:36-41, 362-388   commit, max_degree
 //   plonk_b200::Commitment         src/commitment_scheme/kzg10/commitment.rs:77-106    to_bytes (48 B)
-//   plonk_b200::Prover             src/compiler/prover.rs:53-115, 352-362              prove
-//   plonk_b200::Verifier           src/compiler/verifier.rs:32-262                     verify, to_bytes, try_from_bytes
+//   plonk_b200::Prover             src/compiler/prover.rs:53-115, 352-413              prove, prove_with_version
+//   plonk_b200::Verifier           src/compiler/verifier.rs:32-263                     verify, verify_with_version, to_bytes,
+//                                                                                      try_from_bytes
+//   plonk_b200::PlonkVersion       src/compiler.rs:22-42
 //   plonk_b200::Composer           src/composer.rs:72-495 + src/composer/{bits,range,logic,truncate,select,
 //                                  point,fixed_base}.rs (host-side circuit front end, plonk_b200_composer.h)
 //   plonk_b200::Error              src/error.rs:21-120 (the variants this path can produce)
@@ -34,8 +36,9 @@ struct Error : std::runtime_error {
   enum Kind {
     InvalidEvalDomainSize, PolynomialDegreeTooLarge, CircuitUnsatisfied, InvalidArgument, BackendFailure,
     JubJubPointNotTorsionFree, JubJubGeneratorNotPrimeOrder, JubJubScalarMalformed,
-    ProofVerificationError,  // Error::ProofVerificationError
-    PointMalformed           // Error::BytesError(dusk_bytes::Error::InvalidData) of the verifier's decoders
+    ProofVerificationError,    // Error::ProofVerificationError
+    PointMalformed,            // Error::BytesError(dusk_bytes::Error::InvalidData) of the verifier's decoders
+    UnsupportedProvingVersion  // Error::UnsupportedProvingVersion
   };
   Kind kind;
   Error(Kind k, const std::string& what) : std::runtime_error(what), kind(k) {}
@@ -52,6 +55,7 @@ inline void check(int rc) {
     case PB200_ERR_JUBJUB_POINT: throw Error(Error::JubJubPointNotTorsionFree, msg);
     case PB200_ERR_JUBJUB_GENERATOR: throw Error(Error::JubJubGeneratorNotPrimeOrder, msg);
     case PB200_ERR_JUBJUB_SCALAR: throw Error(Error::JubJubScalarMalformed, msg);
+    case PB200_ERR_UNSUPPORTED_VERSION: throw Error(Error::UnsupportedProvingVersion, msg);
     default: throw Error(Error::BackendFailure, msg);
   }
 }
@@ -323,6 +327,11 @@ inline Circuit circuit_of(const Composer::Export& e) {
   return c;
 }
 
+// PlonkVersion (src/compiler.rs:22-42): V3 is the current profile; V2 is the legacy transcript seed with V3's opening
+// checks; V1 is the legacy seed with the legacy opening, which does not bind the q_arith, q_c, q_l and q_r
+// evaluations, so a V1 verdict is meaningful only for proofs made under the old rules.
+enum class PlonkVersion { V1 = PB200_PLONK_V1, V2 = PB200_PLONK_V2, V3 = PB200_PLONK_V3 };
+
 class Prover {
  public:
   static constexpr size_t PROOF_SIZE = 1008;  // Proof::SIZE
@@ -349,6 +358,16 @@ class Prover {
                       pi_idx.size(), blinders[0].data(), proof.data()));
     return proof;
   }
+  // Prover::prove_with_version: V3 is prove, V2 proves under the legacy transcript seed, V1 throws
+  // UnsupportedProvingVersion.
+  std::array<uint8_t, PROOF_SIZE> prove_with_version(PlonkVersion version, const std::vector<BlsScalar>& witnesses,
+                                                     const std::vector<uint64_t>& pi_idx, const std::vector<BlsScalar>& pi_vals,
+                                                     const std::array<BlsScalar, 14>& blinders) const {
+    std::array<uint8_t, PROOF_SIZE> proof;
+    check(pb200_prove_with_version(h_, (int)version, witnesses[0].data(), witnesses.size(), pi_idx.data(),
+                                   pi_vals.empty() ? nullptr : pi_vals[0].data(), pi_idx.size(), blinders[0].data(), proof.data()));
+    return proof;
+  }
 
  private:
   Prover() : n_witnesses_(0) {}
@@ -356,7 +375,7 @@ class Prover {
   size_t n_witnesses_;
 };
 
-// Verifier (PlonkVersion::V3).  Errors as the reference: verify() throws ProofVerificationError for a proof that
+// Verifier: verify checks PlonkVersion::V3, verify_with_version any version.  Errors as the reference: verify() throws ProofVerificationError for a proof that
 // fails the check, PointMalformed for one Proof::from_bytes refuses, InvalidArgument for a public-input count that
 // is not the verifier's (InconsistentPublicInputsLen); the constructors throw PointMalformed for a degenerate opening
 // key, InvalidArgument for truncated or overflowing bytes (NotEnoughBytes), InvalidEvalDomainSize for a domain of
@@ -388,7 +407,12 @@ class Verifier {
   }
   // Verifier::verify
   void verify(const std::array<uint8_t, PROOF_SIZE>& proof, const std::vector<BlsScalar>& public_inputs) const {
-    const std::vector<int32_t> st = verify_batch({proof}, {public_inputs});
+    verify_with_version(proof, public_inputs, PlonkVersion::V3);
+  }
+  // Verifier::verify_with_version
+  void verify_with_version(const std::array<uint8_t, PROOF_SIZE>& proof, const std::vector<BlsScalar>& public_inputs,
+                           PlonkVersion version) const {
+    const std::vector<int32_t> st = verify_batch({proof}, {public_inputs}, version);
     if (st[0] == PB200_ERR_POINT_MALFORMED) throw Error(Error::PointMalformed, "InvalidData: malformed proof");
     check_verifier(st[0]);
   }
@@ -396,6 +420,11 @@ class Verifier {
   // same number of public inputs.
   std::vector<int32_t> verify_batch(const std::vector<std::array<uint8_t, PROOF_SIZE>>& proofs,
                                     const std::vector<std::vector<BlsScalar>>& public_inputs) const {
+    return verify_batch(proofs, public_inputs, PlonkVersion::V3);
+  }
+  // The same with every proof checked under `version`.
+  std::vector<int32_t> verify_batch(const std::vector<std::array<uint8_t, PROOF_SIZE>>& proofs,
+                                    const std::vector<std::vector<BlsScalar>>& public_inputs, PlonkVersion version) const {
     if (proofs.size() != public_inputs.size()) throw Error(Error::InvalidArgument, "one public-input vector per proof");
     const size_t n_pi = public_inputs.empty() ? 0 : public_inputs[0].size();
     std::vector<BlsScalar> pi;
@@ -404,8 +433,8 @@ class Verifier {
       pi.insert(pi.end(), v.begin(), v.end());
     }
     std::vector<int32_t> st(proofs.size());
-    check_verifier(pb200_verify(h_, proofs.empty() ? nullptr : proofs[0].data(), proofs.size(), pi.empty() ? nullptr : pi[0].data(),
-                                n_pi, st.data()));
+    check_verifier(pb200_verify_with_version(h_, (int)version, proofs.empty() ? nullptr : proofs[0].data(), proofs.size(),
+                                             pi.empty() ? nullptr : pi[0].data(), n_pi, st.data()));
     return st;
   }
 

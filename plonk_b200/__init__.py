@@ -6,8 +6,8 @@ Host-side mirror of the reference's crate-private seam (SURVEY.md section 8b):
     CommitKey.commit                                      reference src/commitment_scheme/kzg10/key.rs:376-388
 
 Everything computes on the GPU through the C ABI in include/plonk_b200.h; there is no CPU path."""
-from ._lib import Pb200Error, lib  # noqa: F401
+from ._lib import Pb200Error, PlonkVersion, lib  # noqa: F401
 from .domain import EvaluationDomain  # noqa: F401
 from .kzg import CommitKey, Commitment, PolynomialDegreeTooLarge  # noqa: F401
-from .prover import CircuitUnsatisfied, Prover  # noqa: F401
+from .prover import CircuitUnsatisfied, Prover, UnsupportedProvingVersion  # noqa: F401
 from .verifier import PointMalformed, ProofVerificationError, Verifier  # noqa: F401

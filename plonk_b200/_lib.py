@@ -4,6 +4,7 @@ Fails loudly when the CUDA library is missing: there is no CPU fallback in the p
 from __future__ import annotations
 
 import ctypes
+import enum
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
@@ -18,6 +19,18 @@ PB200_ERR_INVALID_ARG = -4
 PB200_ERR_UNSATISFIED = -5
 PB200_ERR_POINT_MALFORMED = -10
 PB200_ERR_VERIFY = -11
+PB200_ERR_UNSUPPORTED_VERSION = -12
+
+
+class PlonkVersion(enum.IntEnum):
+    """PlonkVersion (reference src/compiler.rs:22-42), pb200_plonk_version of the C ABI.  V3 is the current
+    profile.  V2 is the legacy transcript seed with V3's opening checks.  V1 is the legacy seed with the legacy
+    opening, which does not bind the q_arith, q_c, q_l and q_r evaluations: its verdict is meaningful only for
+    proofs made under the old rules."""
+
+    V1 = 1
+    V2 = 2
+    V3 = 3
 
 _lib = None
 
@@ -30,7 +43,8 @@ EXPORTS = [
     "pb200_g1_compress", "pb200_g1_decompress", "pb200_raw_commit_key_points", "pb200_commit_key_from_raw_var_bytes", "pb200_g1_add_affine", "pb200_srs_setup_from_secret", "pb200_g1_lagrange_key",
     "pb200_profile_enable", "pb200_throughput_mode", "pb200_profile_read", "pb200_profile_read_sparse",
     "pb200_prover_new", "pb200_prover_from_bytes", "pb200_prover_free", "pb200_prover_commitments", "pb200_prove", "pb200_prove_dev",
-    "pb200_verifier_new", "pb200_verifier_from_bytes", "pb200_verifier_to_bytes", "pb200_verifier_free", "pb200_verify",
+    "pb200_prove_with_version", "pb200_prove_dev_with_version",
+    "pb200_verifier_new", "pb200_verifier_from_bytes", "pb200_verifier_to_bytes", "pb200_verifier_free", "pb200_verify", "pb200_verify_with_version",
     "pb200_imad_peak", "pb200_fp_product_peak", "pb200_selftest_pairing", "pb200_selftest_fr_mul", "pb200_selftest_fp_mul", "pb200_selftest_fp_ops",
 ]
 
@@ -102,6 +116,8 @@ def lib() -> ctypes.CDLL:
         L.pb200_prover_commitments.argtypes = [c.c_void_p, c.c_void_p]
         L.pb200_prove.argtypes = [c.c_void_p, c.c_void_p, c.c_size_t, c.c_void_p, c.c_void_p, c.c_size_t, c.c_void_p, c.c_void_p]
         L.pb200_prove_dev.argtypes = [c.c_void_p, c.c_void_p, c.c_size_t, c.c_void_p, c.c_void_p, c.c_size_t, c.c_void_p, c.c_void_p, c.c_void_p]
+        L.pb200_prove_with_version.argtypes = L.pb200_prove.argtypes[:1] + [c.c_int] + L.pb200_prove.argtypes[1:]
+        L.pb200_prove_dev_with_version.argtypes = L.pb200_prove_dev.argtypes[:1] + [c.c_int] + L.pb200_prove_dev.argtypes[1:]
         L.pb200_srs_setup_from_secret.argtypes = [c.c_void_p, c.c_void_p, c.c_size_t, c.c_void_p]
         L.pb200_profile_enable.argtypes = [c.c_int]
         L.pb200_throughput_mode.argtypes = [c.c_int]
@@ -117,6 +133,7 @@ def lib() -> ctypes.CDLL:
         L.pb200_verifier_free.argtypes = [c.c_void_p]
         L.pb200_verifier_free.restype = None
         L.pb200_verify.argtypes = [c.c_void_p, c.c_void_p, c.c_size_t, c.c_void_p, c.c_size_t, c.c_void_p]
+        L.pb200_verify_with_version.argtypes = [c.c_void_p, c.c_int] + L.pb200_verify.argtypes[1:]
         L.pb200_selftest_pairing.argtypes = [c.c_void_p, c.c_void_p, c.c_size_t, c.c_void_p]
         _bind_composer(L)
         _lib = L

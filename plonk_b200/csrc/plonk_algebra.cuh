@@ -31,7 +31,9 @@ enum Poly { Q_M, Q_L, Q_R, Q_O, Q_F, Q_C, Q_ARITH, Q_RANGE, Q_LOGIC, Q_FIXED, Q_
 // and the commitments in this order, with q_logic before q_range.
 static const int kKeyFileOrder[N_POLY] = {Q_M, Q_L, Q_R, Q_O, Q_F, Q_C, Q_ARITH, Q_LOGIC, Q_RANGE, Q_FIXED, Q_VAR, S1, S2, S3, S4};
 
-// VerifierKey::seed_transcript (widget.rs:218-257) appends the commitments in this order under these labels.
+// VerifierKey::seed_transcript (widget.rs:218-257) appends the commitments in this order under these labels.  The
+// legacy seed of PlonkVersion::V1 and V2 (seed_transcript_legacy) is the same list with one substitution: the
+// commitment of s_sigma_1 goes in under the "s_sigma_4" label, so s_sigma_4 is not bound (transcript.h).
 struct SeedEntry {
   const char* label;
   int poly;

@@ -900,9 +900,10 @@ void prover_free(pb200_prover* P) {
   delete P;
 }
 
-// Prover::prove_inner, V3.  d_wit: n_witnesses Fr on the device; pi_*: host.
-int prove_dev(const pb200_prover* P, const uint64_t* d_wit, const uint64_t* pi_idx, const uint64_t* pi_vals, size_t n_pi,
-              const uint64_t* blinders_host, uint8_t* out_proof, cudaStream_t st) {
+// Prover::prove_inner.  d_wit: n_witnesses Fr on the device; pi_*: host.  version: PB200_PLONK_V3 or V2, which read
+// the same except for the transcript seed (Prover::transcript_for_version, prover.rs:404-413).
+int prove_dev(const pb200_prover* P, int version, const uint64_t* d_wit, const uint64_t* pi_idx, const uint64_t* pi_vals,
+              size_t n_pi, const uint64_t* blinders_host, uint8_t* out_proof, cudaStream_t st) {
   const size_t n = P->n, n8 = P->n8, stride = n + 8;
   const int log_n = P->log_n;
   // With several proofs in flight the dense MSMs give up their latency-oriented bucket splitting (msm.cu)
@@ -921,7 +922,9 @@ int prove_dev(const pb200_prover* P, const uint64_t* d_wit, const uint64_t* pi_i
   }();
   const HFr* BL = (const HFr*)blinders_host;
   // the prover's own constraint count stands for VerifierKey::n
-  pbh::Transcript tr = pbh::seed_transcript(P->label.data(), P->label.size(), P->constraints, P->comm[0], P->constraints);
+  pbh::Transcript tr = version == PB200_PLONK_V3
+                           ? pbh::seed_transcript(P->label.data(), P->label.size(), P->constraints, P->comm[0], P->constraints)
+                           : pbh::seed_transcript_legacy(P->label.data(), P->label.size(), P->constraints, P->comm[0], P->constraints);
   const HFr* PIV = (const HFr*)pi_vals;
   if (n_pi && (!pi_idx || !pi_vals)) return fail(PB200_ERR_INVALID_ARG, "public inputs announced but not given");
   for (size_t i = 0; i < n_pi; i++) {
@@ -1291,8 +1294,22 @@ int pb200_prover_commitments(const pb200_prover_t* p, uint8_t* out /* 15 x 48 */
   return 0;
 }
 
+// Prover::prove_with_version (prover.rs:364-413) before any work: V1 is UnsupportedProvingVersion.
+static int check_proving_version(int version) {
+  if (version == PB200_PLONK_V1) return fail(PB200_ERR_UNSUPPORTED_VERSION, "UnsupportedProvingVersion: PlonkVersion::V1 proofs cannot be made");
+  if (version != PB200_PLONK_V2 && version != PB200_PLONK_V3) return fail(PB200_ERR_INVALID_ARG, "unknown PlonkVersion");
+  return 0;
+}
+
 int pb200_prove(const pb200_prover_t* p, const uint64_t* witnesses, size_t n_witnesses, const uint64_t* pi_idx,
                 const uint64_t* pi_vals, size_t n_pi, const uint64_t* blinders, uint8_t* out_proof) {
+  return pb200_prove_with_version(p, PB200_PLONK_V3, witnesses, n_witnesses, pi_idx, pi_vals, n_pi, blinders, out_proof);
+}
+
+int pb200_prove_with_version(const pb200_prover_t* p, int version, const uint64_t* witnesses, size_t n_witnesses,
+                             const uint64_t* pi_idx, const uint64_t* pi_vals, size_t n_pi, const uint64_t* blinders,
+                             uint8_t* out_proof) {
+  PB_TRY(check_proving_version(version));
   PB_TRY(ensure_init());
   if (!p || !witnesses || !blinders || !out_proof) return fail(PB200_ERR_INVALID_ARG, "null argument");
   if (n_witnesses != p->n_witnesses) return fail(PB200_ERR_INVALID_ARG, "witness count differs from the compiled circuit");
@@ -1304,17 +1321,24 @@ int pb200_prove(const pb200_prover_t* p, const uint64_t* witnesses, size_t n_wit
   if (e != cudaSuccess)
     rc = fail(PB200_ERR_CUDA, "witness upload", cudaGetErrorString(e));
   else
-    rc = prove_dev(p, d_wit, pi_idx, pi_vals, n_pi, blinders, out_proof, st);
+    rc = prove_dev(p, version, d_wit, pi_idx, pi_vals, n_pi, blinders, out_proof, st);
   cudaFreeAsync(d_wit, st);
   return rc;
 }
 
 int pb200_prove_dev(const pb200_prover_t* p, const uint64_t* d_witnesses, size_t n_witnesses, const uint64_t* pi_idx,
                     const uint64_t* pi_vals, size_t n_pi, const uint64_t* blinders, uint8_t* out_proof, void* stream) {
+  return pb200_prove_dev_with_version(p, PB200_PLONK_V3, d_witnesses, n_witnesses, pi_idx, pi_vals, n_pi, blinders, out_proof, stream);
+}
+
+int pb200_prove_dev_with_version(const pb200_prover_t* p, int version, const uint64_t* d_witnesses, size_t n_witnesses,
+                                 const uint64_t* pi_idx, const uint64_t* pi_vals, size_t n_pi, const uint64_t* blinders,
+                                 uint8_t* out_proof, void* stream) {
+  PB_TRY(check_proving_version(version));
   PB_TRY(ensure_init());
   if (!p || !d_witnesses || !blinders || !out_proof) return fail(PB200_ERR_INVALID_ARG, "null argument");
   if (n_witnesses != p->n_witnesses) return fail(PB200_ERR_INVALID_ARG, "witness count differs from the compiled circuit");
   cudaStream_t st = stream ? (cudaStream_t)stream : thread_stream();
-  return prove_dev(p, d_witnesses, pi_idx, pi_vals, n_pi, blinders, out_proof, st);
+  return prove_dev(p, version, d_witnesses, pi_idx, pi_vals, n_pi, blinders, out_proof, st);
 }
 }

@@ -136,18 +136,34 @@ class Transcript {
   Strobe128 s_;
 };
 
-// ---- The V3 schedule: what goes into the transcript, in which order, under which label ----------------------
-// Prover::prove_inner (prover.rs:415-761) and Proof::verify (proof.rs:218-300) run the same sequence.  The
-// commitments are read from `comms`, the 11 compressed commitments in Proof::to_bytes order.
+// ---- The schedule: what goes into the transcript, in which order, under which label --------------------------
+// Prover::prove_inner (prover.rs:415-761), Proof::verify (proof.rs:218-300) and Proof::verify_legacy
+// (proof.rs:540-614) run the same sequence; the versions differ only in the seed.  The commitments are read from
+// `comms`, the 11 compressed commitments in Proof::to_bytes order.
 
-// Transcript::base (transcript.rs:131-145) with VerifierKey::seed_transcript (widget.rs:218-257).  key_comms: the 15
-// key commitments in pb::Poly order; vk_n: VerifierKey::n, which seed_transcript_inner appends last.
-inline Transcript seed_transcript(const uint8_t* label, size_t label_len, uint64_t constraints, const uint8_t* key_comms, uint64_t vk_n) {
+// VerifierKey::seed_transcript_inner (widget.rs:218-257) after Transcript::new and the constraint count.  key_comms:
+// the 15 key commitments in pb::Poly order; vk_n: VerifierKey::n, which it appends last.  bind_s_sigma_4 = false
+// is the legacy seed: s_sigma_1's commitment goes in under the "s_sigma_4" label (pb::kSeedOrder).
+inline Transcript seed_transcript_inner(const uint8_t* label, size_t label_len, uint64_t constraints, const uint8_t* key_comms,
+                                        uint64_t vk_n, bool bind_s_sigma_4) {
   Transcript tr(label, label_len);
   tr.circuit_domain_sep(constraints);
-  for (const pb::SeedEntry& s : pb::kSeedOrder) tr.append_commitment(s.label, key_comms + 48 * s.poly);
+  for (const pb::SeedEntry& s : pb::kSeedOrder) {
+    const int poly = s.poly == pb::S4 && !bind_s_sigma_4 ? pb::S1 : s.poly;
+    tr.append_commitment(s.label, key_comms + 48 * poly);
+  }
   tr.circuit_domain_sep(vk_n);
   return tr;
+}
+// Transcript::base_v3 (transcript.rs:131-145) with VerifierKey::seed_transcript: PlonkVersion::V3.
+inline Transcript seed_transcript(const uint8_t* label, size_t label_len, uint64_t constraints, const uint8_t* key_comms, uint64_t vk_n) {
+  return seed_transcript_inner(label, label_len, constraints, key_comms, vk_n, true);
+}
+// Transcript::base (transcript.rs:110-129) with VerifierKey::seed_transcript_legacy (widget.rs:259-265):
+// PlonkVersion::V1 and V2.
+inline Transcript seed_transcript_legacy(const uint8_t* label, size_t label_len, uint64_t constraints, const uint8_t* key_comms,
+                                         uint64_t vk_n) {
+  return seed_transcript_inner(label, label_len, constraints, key_comms, vk_n, false);
 }
 // The wire commitments -> beta, gamma.
 inline void challenge_beta_gamma(Transcript& tr, const uint8_t* comms, pb::Challenges& c) {

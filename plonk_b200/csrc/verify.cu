@@ -1,10 +1,12 @@
-// Verifier (reference src/compiler/verifier.rs) for PlonkVersion::V3 proofs: Verifier::verify for a batch of proofs
-// per call, one verdict per proof.
+// Verifier (reference src/compiler/verifier.rs): Verifier::verify_with_version for a batch of proofs per call, one
+// verdict per proof, for PlonkVersion V1, V2 and V3.
 //
 // The host parses, replays the transcript and computes the O(#public inputs) scalars of Proof::verify
-// (src/proof_system/proof.rs:218-516).  The device decodes the commitments (k_g1_decompress), forms the two G1
-// points of the final pairing check with one warp per proof (k_verify_msm), and runs the multi-Miller loop, the
-// final exponentiation and the comparison with 1 with one thread per proof (k_verify_pairing).
+// (src/proof_system/proof.rs:218-516) or, for V1, Proof::verify_legacy (proof.rs:518-790); see verify_scalars.h.
+// The device decodes the commitments (k_g1_decompress), forms the two G1 points of the final pairing check with one
+// warp per proof (k_verify_msm), and runs the multi-Miller loop, the final exponentiation and the comparison with 1
+// with one thread per proof (k_verify_pairing).  The device work is the same for every version: V1 only gives the
+// four selector-opening terms zero scalars.
 #include <algorithm>
 #include <mutex>
 #include <thread>
@@ -16,20 +18,18 @@
 #include "pairing.cuh"
 #include "plonk_algebra.cuh"
 #include "transcript.h"
+#include "verify_scalars.h"
 
 struct pb200_verifier {
   std::vector<uint8_t> label;
   uint64_t vk_n = 0;                          // VerifierKey::n: the constraint count for a compiled circuit
-  uint64_t n = 0, size = 0, constraints = 0;  // the domain size (EvaluationDomain::new(vk_n)), Verifier::size, Verifier::constraints
+  uint64_t size = 0, constraints = 0;         // Verifier::size, Verifier::constraints
   uint8_t vk_comm[pb::N_POLY][48];             // pb::Poly order
   uint8_t opening_key[PB200_OPENING_KEY_BYTES];
   std::vector<uint64_t> pi_idx;
-  std::vector<pbh::HFr> pi_roots;  // group_gen_inv^index
-  pbh::HFr group_gen, size_fr, size_inv;
-  pbh::Transcript base;
+  pb::VerifyKeyHost key;            // both base transcripts, the domain (EvaluationDomain::new(vk_n)) and the pi roots
   uint4* d_points = nullptr;        // the 15 key commitments then opening_key.g, 96-byte raw affine
   pb::LineCoeffs* d_lines = nullptr;  // prepared [x]H then H, PB_G2_LINES each
-  pb200_verifier() : base(nullptr, 0) {}
 };
 
 namespace pb {
@@ -80,7 +80,6 @@ PB_D G1Affine to_affine(const G1Xyzz& p) {
 enum { P_A = 16, P_B, P_C, P_D, P_Z, P_TLOW, P_TMID, P_THIGH, P_TFOURTH, P_WZ, P_WZW };
 __constant__ int c_term_point[32] = {0,  1,  2,  3,       4,      5,      7,       8,         9,    10, P_Z,   14, P_TLOW, P_TMID, P_THIGH, P_TFOURTH,
                                      P_A, P_B, P_C, P_D, 11, 12, 13, 6, 5, 1, 2, 15, P_WZ, P_WZW, -1, P_WZW};
-#define PB_VERIFY_TERMS 32
 
 // One warp per proof.  scalars: [proof][32] canonical little-endian Fr; proof_comm: [proof][11] compressed
 // commitments; pts: their decoded points.  status: PB200_OK on entry or the host's verdict; a commitment that
@@ -206,92 +205,6 @@ int g2_prepare_dev(const uint8_t* enc, int count, LineCoeffs* d_lines, int* ok, 
   return 0;
 }
 
-bool fr_canonical(const uint8_t* b, HFr* out) {  // BlsScalar::from_bytes: little-endian, below r
-  uint64_t w[4];
-  memcpy(w, b, 32);
-  for (int k = 3; k >= 0; k--) {
-    if (w[k] < pbh::kFrMod.p[k]) break;
-    if (w[k] > pbh::kFrMod.p[k] || k == 0) return false;
-  }
-  memcpy(out->v, w, 32);
-  *out = out->to_mont();
-  return true;
-}
-
-// Proof::verify up to the pairing: the transcript replay and the 32 scalars of k_verify_msm (canonical form).
-// Returns PB200_OK, PB200_ERR_POINT_MALFORMED for a non-canonical evaluation or PB200_ERR_VERIFY.
-int verify_scalars(const pb200_verifier* V, const uint8_t* proof, const HFr* pi, uint64_t* out) {
-  HFr e[N_EVAL];
-  for (int k = 0; k < N_EVAL; k++)
-    if (!fr_canonical(proof + kProofEvalAt + 32 * k, &e[k])) return PB200_ERR_POINT_MALFORMED;
-  pbh::Transcript tr = V->base;
-  for (size_t k = 0; k < V->pi_idx.size(); k++) tr.append_scalar("pi", pi[k]);
-  Challenges c;
-  pbh::challenge_beta_gamma(tr, proof, c);
-  pbh::challenge_alpha(tr, proof, c);
-  pbh::challenge_z(tr, proof, c);
-  pbh::challenge_v(tr, e, c);
-  pbh::challenge_u(tr, proof, c);
-  const HFr &z = c.z, &v = c.v, &v_w = c.v_w, &u = c.u;
-
-  const HFr one = HFr::one();
-  const HFr z_n = z.pow_u64(V->n), z_h = z_n - one;
-  // compute_lagrange_and_barycentric_evaluations (proof.rs:997-1040): one batch inversion
-  std::vector<HFr> den, pref;
-  std::vector<size_t> which;
-  den.push_back(V->size_fr * (z - one));
-  for (size_t k = 0; k < V->pi_idx.size(); k++)
-    if (!pi[k].is_zero()) {
-      den.push_back(V->pi_roots[k] * z - one);
-      which.push_back(k);
-    }
-  pref.resize(den.size());
-  HFr acc = one;
-  for (size_t k = 0; k < den.size(); k++) {
-    if (den[k].is_zero()) return PB200_ERR_VERIFY;
-    pref[k] = acc;
-    acc = acc * den[k];
-  }
-  HFr inv = acc.inv_bingcd();
-  for (size_t k = den.size(); k-- > 0;) {
-    const HFr d = den[k];
-    den[k] = inv * pref[k];
-    inv = inv * d;
-  }
-  const HFr l1 = z_h * den[0];
-  HFr pi_eval = HFr::zero();
-  for (size_t j = 0; j < which.size(); j++) pi_eval = pi_eval + den[1 + j] * pi[which[j]];
-  pi_eval = pi_eval * z_h * V->size_inv;
-
-  const HFr perm = perm_copy3(eval_wires(e), c.beta, c.gamma, [&](int j) { return e[E_S1 + j]; });
-  const HFr r0 = pi_eval - l1 * c.alpha.sqr() - c.alpha * perm * (e[E_D] + c.gamma) * e[E_Z];
-  HFr vc[14];
-  vc[0] = v;
-  for (int k = 1; k < 11; k++) vc[k] = vc[k - 1] * v;
-  vc[11] = v_w * u;
-  vc[12] = vc[11] * v_w;
-  vc[13] = vc[12] * v_w;
-  const int eo[14] = {E_A, E_B, E_C, E_D, E_S1, E_S2, E_S3, E_QARITH, E_QC, E_QL, E_QR, E_AW, E_BW, E_DW};
-  HFr E = u * e[E_Z] - r0;
-  for (int k = 0; k < 14; k++) E = E + e[eo[k]] * vc[k];
-
-  const LinScalars ls = linearisation_scalars(e, c, z_n, l1);
-  HFr f[11];
-  for (int k = 0; k < 11; k++) f[k] = vc[k];
-  f[0] = f[0] + vc[11];
-  f[1] = f[1] + vc[12];
-  f[3] = f[3] + vc[13];
-  const HFr s[PB_VERIFY_TERMS] = {ls.sel[Q_M], ls.sel[Q_L], ls.sel[Q_R], ls.sel[Q_O], ls.sel[Q_F], ls.sel[Q_C], ls.sel[Q_RANGE],
-                                  ls.sel[Q_LOGIC], ls.sel[Q_FIXED], ls.sel[Q_VAR], ls.z + u, ls.sel[S4], ls.t[0], ls.t[1], ls.t[2],
-                                  ls.t[3], f[0], f[1], f[2], f[3], f[4], f[5], f[6], f[7], f[8], f[9], f[10],
-                                  E.neg(), z, u * z * V->group_gen, HFr::zero(), u};
-  for (int k = 0; k < PB_VERIFY_TERMS; k++) {
-    const HFr cn = s[k].from_mont();
-    memcpy(out + 4 * k, cn.v, 32);
-  }
-  return PB200_OK;
-}
-
 uint64_t be64(const uint8_t* b) {
   uint64_t x = 0;
   for (int k = 0; k < 8; k++) x = (x << 8) | b[k];
@@ -338,7 +251,6 @@ int verifier_build(const uint8_t* label, size_t label_len, uint64_t vk_n, uint64
   V->d_lines = d_lines;
   V->label.assign(label, label + label_len);
   V->vk_n = vk_n;
-  V->n = (uint64_t)1 << log_n;
   V->size = size;
   V->constraints = constraints;
   memcpy(V->vk_comm, comms, 15 * 48);
@@ -351,12 +263,16 @@ int verifier_build(const uint8_t* label, size_t label_len, uint64_t vk_n, uint64
   for (int k = 0; k < 4; k++) t[k] = (t[k] >> 32) | (k < 3 ? t[k + 1] << 32 : 0);
   HFr g = HFr::from_u64(7).pow(t, 4);
   for (int k = log_n; k < 32; k++) g = g.sqr();
-  V->group_gen = g;
-  V->size_fr = HFr::from_u64(V->n);
-  V->size_inv = V->size_fr.inv();
+  VerifyKeyHost& K = V->key;
+  K.n = (uint64_t)1 << log_n;
+  K.group_gen = g;
+  K.size_fr = HFr::from_u64(K.n);
+  K.size_inv = K.size_fr.inv();
   const HFr g_inv = g.inv();
-  for (uint64_t idx : V->pi_idx) V->pi_roots.push_back(g_inv.pow_u64(idx));
-  V->base = pbh::seed_transcript(V->label.data(), V->label.size(), constraints, comms, vk_n);
+  for (uint64_t idx : V->pi_idx) K.pi_roots.push_back(g_inv.pow_u64(idx));
+  // Verifier::transcript (Transcript::base, V1 and V2) and Transcript::base_v3 (V3): built once for every version
+  K.base_v3 = pbh::seed_transcript(V->label.data(), V->label.size(), constraints, comms, vk_n);
+  K.base_legacy = pbh::seed_transcript_legacy(V->label.data(), V->label.size(), constraints, comms, vk_n);
   cudaError_t e = cudaMalloc((void**)&V->d_points, 16 * 96);
   if (e == cudaSuccess) e = cudaMemcpy(V->d_points, raw.data(), 16 * 96, cudaMemcpyHostToDevice);
   if (e != cudaSuccess) {
@@ -449,8 +365,15 @@ void pb200_verifier_free(pb200_verifier_t* V) {
 
 int pb200_verify(const pb200_verifier_t* V, const uint8_t* proofs, size_t n_proofs, const uint64_t* pi_vals, size_t n_pi,
                  int32_t* status) {
+  return pb200_verify_with_version(V, PB200_PLONK_V3, proofs, n_proofs, pi_vals, n_pi, status);
+}
+
+int pb200_verify_with_version(const pb200_verifier_t* V, int version, const uint8_t* proofs, size_t n_proofs,
+                              const uint64_t* pi_vals, size_t n_pi, int32_t* status) {
   PB_TRY(ensure_init());
   if (!V || (!proofs && n_proofs) || (!pi_vals && n_pi && n_proofs) || (!status && n_proofs)) return fail(PB200_ERR_INVALID_ARG, "null argument");
+  if (version != PB200_PLONK_V1 && version != PB200_PLONK_V2 && version != PB200_PLONK_V3)
+    return fail(PB200_ERR_INVALID_ARG, "unknown PlonkVersion");
   if (n_pi != V->pi_idx.size()) return fail(PB200_ERR_INVALID_ARG, "InconsistentPublicInputsLen");
   if (!n_proofs) return 0;
   PB_TRY(upload_pairing_consts());
@@ -462,7 +385,7 @@ int pb200_verify(const pb200_verifier_t* V, const uint8_t* proofs, size_t n_proo
     for (size_t i = lo; i < hi; i++) {
       const uint8_t* pr = proofs + kProofBytes * i;
       memcpy(comm.data() + kProofEvalAt * i, pr, kProofEvalAt);
-      hstat[i] = verify_scalars(V, pr, (const HFr*)(pi_vals + 4 * n_pi * i), scal.data() + (size_t)PB_VERIFY_TERMS * 4 * i);
+      hstat[i] = verify_scalars(V->key, version, pr,(const HFr*)(pi_vals + 4 * n_pi * i), scal.data() + (size_t)PB_VERIFY_TERMS * 4 * i);
     }
   };
   const size_t n_thr = std::min<size_t>(std::max(1u, std::thread::hardware_concurrency()), std::min<size_t>(16, (n_proofs + 31) / 32));

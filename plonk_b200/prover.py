@@ -1,5 +1,5 @@
-"""Prover mirror (reference src/compiler/prover.rs: Prover::new :53-115, Prover::prove :352-362)
-over the device-resident CUDA prover.
+"""Prover mirror (reference src/compiler/prover.rs: Prover::new :53-115, Prover::prove :352-362,
+Prover::prove_with_version :364-413) over the device-resident CUDA prover.
 
 A circuit crosses the boundary as flat arrays, i.e. what Compiler::preprocess reads out of the
 Composer (reference src/compiler.rs:132-170): 11 selector columns, 4 wire columns, the witness
@@ -8,13 +8,17 @@ from __future__ import annotations
 
 import ctypes
 
-from ._lib import PB200_ERR_UNSATISFIED, Pb200Error, check, lib
+from ._lib import PB200_ERR_UNSATISFIED, PB200_ERR_UNSUPPORTED_VERSION, Pb200Error, PlonkVersion, check, lib
 
 PROOF_BYTES = 1008
 
 
 class CircuitUnsatisfied(ValueError):
     """Error::CircuitUnsatisfied (reference src/proof_system/quotient_poly.rs:132-134)."""
+
+
+class UnsupportedProvingVersion(ValueError):
+    """Error::UnsupportedProvingVersion: PlonkVersion::V1 proofs cannot be made (reference prover.rs:376)."""
 
 
 class Prover:
@@ -45,15 +49,24 @@ class Prover:
         return [out.raw[48 * i : 48 * i + 48] for i in range(15)]
 
     def prove(self, witnesses: bytes, pi_idx: bytes, pi_vals: bytes, blinders: bytes) -> bytes:
-        """witnesses: n_witnesses x 32 B; pi_idx: u64 LE positions; pi_vals: 32 B each; blinders: 14 x 32 B."""
+        """Prover::prove (PlonkVersion::V3).  witnesses: n_witnesses x 32 B; pi_idx: u64 LE positions; pi_vals: 32 B
+        each; blinders: 14 x 32 B."""
+        return self.prove_with_version(PlonkVersion.V3, witnesses, pi_idx, pi_vals, blinders)
+
+    def prove_with_version(self, version: PlonkVersion, witnesses: bytes, pi_idx: bytes, pi_vals: bytes, blinders: bytes) -> bytes:
+        """Prover::prove_with_version: as prove, under `version`.  V3 is prove; V2 uses the legacy transcript seed;
+        V1 raises UnsupportedProvingVersion; any other value is a Pb200Error with PB200_ERR_INVALID_ARG."""
         assert len(blinders) == 14 * 32 and len(witnesses) == self.n_witnesses * 32
         n_pi = len(pi_idx) // 8
         out = ctypes.create_string_buffer(PROOF_BYTES)
         try:
-            check(lib().pb200_prove(self._h, witnesses, self.n_witnesses, pi_idx or None, pi_vals or None, n_pi, blinders, out))
+            check(lib().pb200_prove_with_version(self._h, int(version), witnesses, self.n_witnesses, pi_idx or None, pi_vals or None,
+                                                 n_pi, blinders, out))
         except Pb200Error as e:
             if e.code == PB200_ERR_UNSATISFIED:
                 raise CircuitUnsatisfied() from e
+            if e.code == PB200_ERR_UNSUPPORTED_VERSION:
+                raise UnsupportedProvingVersion("UnsupportedProvingVersion") from e
             raise
         return out.raw
 

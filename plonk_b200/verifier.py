@@ -1,11 +1,12 @@
-"""Verifier (reference src/compiler/verifier.rs, PlonkVersion::V3) on the GPU, through pb200_verifier_* and
-pb200_verify of include/plonk_b200.h."""
+"""Verifier (reference src/compiler/verifier.rs) on the GPU, through pb200_verifier_* and
+pb200_verify_with_version of include/plonk_b200.h.  Every PlonkVersion is verified on the device; V3 is the
+default."""
 from __future__ import annotations
 
 import ctypes
 from typing import List, Sequence
 
-from ._lib import PB200_ERR_INVALID_ARG, PB200_ERR_POINT_MALFORMED, PB200_ERR_VERIFY, Pb200Error, check, lib
+from ._lib import PB200_ERR_INVALID_ARG, PB200_ERR_POINT_MALFORMED, PB200_ERR_VERIFY, Pb200Error, PlonkVersion, check, lib
 
 PROOF_BYTES = 1008
 OPENING_KEY_BYTES = 240
@@ -48,22 +49,27 @@ class Verifier:
         check(lib().pb200_verifier_to_bytes(self._h, out, n.value, ctypes.byref(n)))
         return out.raw
 
-    def verify_batch(self, proofs: Sequence[bytes], pi_vals: Sequence[bytes]) -> List[int]:
+    def verify_batch(self, proofs: Sequence[bytes], pi_vals: Sequence[bytes], version: PlonkVersion = PlonkVersion.V3) -> List[int]:
         """One status per proof (PB200_OK, PB200_ERR_VERIFY or PB200_ERR_POINT_MALFORMED); pi_vals[i]: the public
-        inputs of proof i, 32 bytes (Montgomery form) each."""
+        inputs of proof i, 32 bytes (Montgomery form) each.  Every proof is checked under `version`."""
         assert len(proofs) == len(pi_vals) and all(len(p) == PROOF_BYTES for p in proofs)
         n_pi = len(pi_vals[0]) // 32 if pi_vals else self.n_pi
         if any(len(v) != 32 * n_pi for v in pi_vals):
             raise ValueError("every proof needs the same number of public inputs")
         status = (ctypes.c_int32 * max(1, len(proofs)))()
         vals = b"".join(pi_vals)
-        check(lib().pb200_verify(self._h, b"".join(proofs), len(proofs), vals or None, n_pi, status))
+        check(lib().pb200_verify_with_version(self._h, int(version), b"".join(proofs), len(proofs), vals or None, n_pi, status))
         return list(status[: len(proofs)])
 
     def verify(self, proof: bytes, pi_vals: bytes) -> None:
         """Verifier::verify: returns on success, raises ProofVerificationError, PointMalformed or ValueError."""
+        self.verify_with_version(proof, pi_vals, PlonkVersion.V3)
+
+    def verify_with_version(self, proof: bytes, pi_vals: bytes, version: PlonkVersion) -> None:
+        """Verifier::verify_with_version: as verify, under `version`.  A V1 verdict does not bind the selector
+        evaluations; it is meaningful only for proofs made under the old rules."""
         try:
-            (st,) = self.verify_batch([proof], [pi_vals])
+            (st,) = self.verify_batch([proof], [pi_vals], version)
         except Pb200Error as e:
             if e.code == PB200_ERR_INVALID_ARG:
                 raise ValueError(str(e)) from e
