@@ -217,6 +217,19 @@ struct Field {
 #pragma unroll
     for (int i = 0; i < N; i++) r[i] = ge ? s[i] : t[i];
   }
+  // The end of a Montgomery product whose pre-subtraction value t is < 2p: reduced to [0, p) when FULL,
+  // left as it is for FpR otherwise.
+  template <bool FULL>
+  static PB_HD Field finish(const uint32_t* t) {
+    Field r;
+    if (FULL) {
+      final_sub(r.v, t, 0u);
+    } else {
+#pragma unroll
+      for (int i = 0; i < N; i++) r.v[i] = t[i];
+    }
+    return r;
+  }
 
   friend PB_HD Field operator+(const Field& a, const Field& b) {
     uint32_t t[N];
@@ -309,12 +322,16 @@ struct Field {
     red_row(X, Y);
   }
 
-  friend PB_HD Field operator*(const Field& a, const Field& b) {
+  friend PB_HD Field operator*(const Field& a, const Field& b) { return mul<true>(a, b); }
+  // FULL = false skips the final subtraction (FpR: operands < 2p give a result < 2p, see there).
+  template <bool FULL>
+  static PB_HD Field mul(const Field& a, const Field& b) {
 #if defined(__CUDA_ARCH__)
-    if constexpr (P::HYBRID) return mul_hybrid(a, b);
+    if constexpr (P::HYBRID) return mul_hybrid<FULL>(a, b);
 #endif
-    return mul_imad(a, b);
+    return mul_imad<FULL>(a, b);
   }
+  template <bool FULL = true>
   static PB_HD Field mul_imad(const Field& a, const Field& b) {
     uint32_t A[N], B[N];
     {
@@ -338,17 +355,16 @@ struct Field {
 #pragma unroll
     for (int k = 1; k < N - 1; k++) t[k] = addc_cc(A[k], B[k + 1]);
     t[N - 1] = addc(A[N - 1], 0u);
-    Field r;
-    final_sub(r.v, t, 0u);
-    return r;
+    return finish<FULL>(t);
   }
   // Squaring with the symmetric partial products taken once: a^2 = sum_i a_i * B_i with
   // B_i = a_i 2^(32i) + 2 sum_{k>i} a_k 2^(32k), so row i multiplies a_i only by the limbs k >= i of
   // the doubled operand (N(N+1)/2 multiply-adds instead of N^2; the Montgomery steps are unchanged).
   // The skipped links of the shifting accumulator become plain carry-propagating adds.
   // Row 0 adds a_0 * 2a at once, twice what a row of the ordinary product adds, so the running sum
-  // needs 3p * 2^32 < 2^(32(N+1)): two spare bits in the top limb.  Fp has three; Fr (one) keeps the
-  // ordinary product.
+  // needs (2a + p) * 2^32 < 2^(32(N+1)): 3p for a < p, 5p for an FpR operand a < 2p.  Both need two
+  // spare bits in the top limb (and 2a must fit N limbs).  Fp has three; Fr (one) keeps the ordinary
+  // product.
   template <int I>
   static PB_HD uint32_t sq_limb(const uint32_t* a, const uint32_t* a2, int k) {
     return k == I ? a[k] : (k == I + 1 ? (a[k] << 1) : a2[k]);
@@ -387,16 +403,18 @@ struct Field {
       sqr_rows<I + 2>(A, B, a, a2);
     }
   }
+  template <bool FULL = true>
   PB_HD Field sqr() const {
 #if defined(__CUDA_ARCH__)
-    if constexpr (P::HYBRID && (P::MOD(N - 1) >> 30) == 0) return sqr_hybrid();
+    if constexpr (P::HYBRID && (P::MOD(N - 1) >> 30) == 0) return sqr_hybrid<FULL>();
 #endif
     if constexpr ((P::MOD(N - 1) >> 30) != 0) {
-      return (*this) * (*this);
+      return mul<FULL>(*this, *this);
     } else {
-      return sqr_half();
+      return sqr_half<FULL>();
     }
   }
+  template <bool FULL = true>
   PB_HD Field sqr_half() const {
     static_assert((P::MOD(N - 1) >> 30) == 0, "needs two spare bits in the top limb of the modulus");
     uint32_t a2[N];
@@ -419,21 +437,24 @@ struct Field {
 #pragma unroll
     for (int k = 1; k < N - 1; k++) t[k] = addc_cc(A[k], B[k + 1]);
     t[N - 1] = addc(A[N - 1], 0u);
-    Field r;
-    final_sub(r.v, t, 0u);
-    return r;
+    return finish<FULL>(t);
   }
 
   // a*b + c*d with ONE Montgomery reduction: each row accumulates both partial products before its
   // Montgomery step (3N^2 multiply-adds instead of 4N^2).  Only for moduli with at least two spare
   // bits in the top limb (Fp: 381 of 384 bits), where the running sum keeps fitting the two
   // accumulators and the result stays below 2p; Fr (255 of 256 bits) must not use it.
+  // The running sum entering a row is < a + c + p, so a row peaks below (a + c + p) * 2^32: 3p for
+  // canonical operands, 5p for FpR operands (all four < 2p), inside 2^(32(N+1)) when 8p < 2^(32N).
+  // The result is < p + (ab + cd) / 2^(32N) < p + 8p^2 / 2^(32N) < 2p in both cases.
+  template <bool FULL = true>
   static PB_HD Field mul2(const Field& a, const Field& b, const Field& c, const Field& d) {
 #if defined(__CUDA_ARCH__)
-    if constexpr (P::HYBRID) return mul2_hybrid(a, b, c, d);
+    if constexpr (P::HYBRID) return mul2_hybrid<FULL>(a, b, c, d);
 #endif
-    return mul2_imad(a, b, c, d);
+    return mul2_imad<FULL>(a, b, c, d);
   }
+  template <bool FULL = true>
   static PB_HD Field mul2_imad(const Field& a, const Field& b, const Field& c, const Field& d) {
     static_assert((P::MOD(N - 1) >> 30) == 0, "mul2 needs two spare bits in the top limb of the modulus");
     uint32_t A[N], B[N];
@@ -464,9 +485,7 @@ struct Field {
 #pragma unroll
     for (int k = 1; k < N - 1; k++) t[k] = addc_cc(A[k], B[k + 1]);
     t[N - 1] = addc(A[N - 1], 0u);
-    Field r;
-    final_sub(r.v, t, 0u);
-    return r;
+    return finish<FULL>(t);
   }
   // -------------------------------------------------------------------------------------------
   // Two-pipe ("hybrid") product (Fp: 384 bits = 8 x 48; Fr: 256 bits = 5 x 48 + 16).
@@ -495,7 +514,8 @@ struct Field {
     return (uint64_t)npairs48(k) * 0x4330000000000000ull + (uint64_t)npairs48(k - 1) * 0x4630000000000000ull;
   }
   static PB_HD uint32_t word_or_zero(const uint32_t* T, int k) { return k < 2 * N ? T[k] : 0u; }
-  // T[2N] * 2^(-32N) mod p for T < p * 2^(32N), fully reduced.
+  // T[2N] * 2^(-32N) mod p for T < p * 2^(32N): fully reduced when FULL, else < 2p (FpR).
+  template <bool FULL>
   static PB_HD Field redc48(const uint32_t* T) {
     uint64_t c[2 * L48];
     // T[2N-1] has at least two spare bits, so `gate` is zero - but ptxas cannot know, which keeps it
@@ -559,9 +579,7 @@ struct Field {
       else
         t[w] = (uint32_t)(c[k] >> 32) | ((uint32_t)c[k + 1] << 16);
     }
-    Field res;
-    final_sub(res.v, t, 0u);
-    return res;
+    return finish<FULL>(t);
   }
   // E = B (low word already out), O = A after the last row: upper half T[N..2N) = A + (B >> 32)
   static PB_HD void wide_top(uint32_t* T, const uint32_t* A, const uint32_t* B) {
@@ -622,23 +640,28 @@ struct Field {
     wide_sqr_rows<1>(T, A, B, v, a2);
     wide_top(T, A, B);
   }
+  // FpR operands (< 2p) give T < 8p^2 < p * 2^(32N) with three spare bits, and T[2N-1] keeps two
+  // zero top bits (8p^2 < 2^765 for Fp), which `gate` relies on.
+  template <bool FULL = true>
   static PB_HD Field mul_hybrid(const Field& a, const Field& b) {
     uint32_t T[2 * N];
     wide_mul<false>(T, a.v, b.v, a.v, b.v);
-    return redc48(T);
+    return redc48<FULL>(T);
   }
+  template <bool FULL = true>
   PB_HD Field sqr_hybrid() const {
     static_assert((P::MOD(N - 1) >> 30) == 0, "needs two spare bits in the top limb of the modulus");
     uint32_t T[2 * N];
     wide_sqr(T, v);
-    return redc48(T);
+    return redc48<FULL>(T);
   }
   // a*b + c*d < 2p^2 < p * 2^(32N) needs one spare bit
+  template <bool FULL = true>
   static PB_HD Field mul2_hybrid(const Field& a, const Field& b, const Field& c, const Field& d) {
     static_assert((P::MOD(N - 1) >> 30) == 0, "needs two spare bits in the top limb of the modulus");
     uint32_t T[2 * N];
     wide_mul<true>(T, a.v, b.v, c.v, d.v);
-    return redc48(T);
+    return redc48<FULL>(T);
   }
 
   // a*b - c*d
@@ -748,5 +771,118 @@ struct FpParams {
 
 typedef Field<FrParams> Fr;
 typedef Field<FpParams> Fp;
+
+// ---------------------------------------------------------------------------------------------
+// FpR: an Fp residue kept in [0, 2p) instead of [0, p) (Montgomery form, R = 2^384), for the G1
+// formulas of the MSM.  p < 2^381, so 8p < R, and a Montgomery product returns
+//     (a b + m p) / R < p + a b / R,      m < R,
+// which is < 2p whenever a b < p R, i.e. for any two operands below 2p (4p^2 < 8p^2 < p R).  So
+// products, squares and mul2 / mul_sub of FpR values need no final subtraction - about 25 of the
+// ~1100 instructions of a product.  The running sums of the product rows stay inside the two
+// accumulators (each row peaks below (operand bound + p) * 2^32, at most 5p * 2^32 < 2^416; see
+// Field::sqr_half and Field::mul2 for the squaring's doubled row 0 and the fused pair).
+// Additions and subtractions reduce by 2p and cost what the canonical ones cost.  A residue has up to
+// two representations, so equality with zero is is_zero_mod_p(); canonical() is the one way back to Fp.
+// Canonical Fp (pairing, decoders, host) is untouched.
+// ---------------------------------------------------------------------------------------------
+struct FpR {
+  static constexpr int N = 12;
+  static_assert((FpParams::MOD(N - 1) >> 29) == 0, "FpR needs 8p < 2^384");
+  uint32_t v[N];
+
+  static PB_HD constexpr uint32_t MOD2(int i) {  // 2p
+    return (FpParams::MOD(i) << 1) | (i > 0 ? FpParams::MOD(i - 1) >> 31 : 0u);
+  }
+  // limbs < 2p taken as they are: a canonical Fp, or the result of a product routine run without its
+  // final subtraction
+  static PB_HD FpR from(const Fp& a) {
+    FpR r;
+#pragma unroll
+    for (int i = 0; i < N; i++) r.v[i] = a.v[i];
+    return r;
+  }
+  static PB_HD FpR zero() { return from(Fp::zero()); }
+  static PB_HD FpR one() { return from(Fp::one()); }
+  // [0, 2p) -> [0, p)
+  PB_HD Fp canonical() const {
+    Fp r;
+    Fp::final_sub(r.v, v, 0u);
+    return r;
+  }
+  // the limbs read as an Fp operand of the product routines (which accept operands < 2p, see above)
+  PB_HD Fp raw() const {
+    Fp r;
+#pragma unroll
+    for (int i = 0; i < N; i++) r.v[i] = v[i];
+    return r;
+  }
+  // all limbs zero: the representation 0 only (p is the other representation of zero)
+  PB_HD bool is_zero_limbs() const {
+    uint32_t x = 0;
+#pragma unroll
+    for (int i = 0; i < N; i++) x |= v[i];
+    return x == 0;
+  }
+  // == 0 mod p: the value is 0 or p
+  PB_HD bool is_zero_mod_p() const {
+    uint32_t z = 0, q = 0;
+#pragma unroll
+    for (int i = 0; i < N; i++) {
+      z |= v[i];
+      q |= v[i] ^ FpParams::MOD(i);
+    }
+    return z == 0 || q == 0;
+  }
+
+  // a + b < 4p < 2^384 (no carry out of the top limb); one conditional subtraction of 2p -> [0, 2p)
+  friend PB_HD FpR operator+(const FpR& a, const FpR& b) {
+    uint32_t t[N], s[N];
+    t[0] = add_cc(a.v[0], b.v[0]);
+#pragma unroll
+    for (int i = 1; i < N; i++) t[i] = addc_cc(a.v[i], b.v[i]);
+    s[0] = sub_cc(t[0], MOD2(0));
+#pragma unroll
+    for (int i = 1; i < N; i++) s[i] = subc_cc(t[i], MOD2(i));
+    const bool ge = subc(0u, 0u) == 0u;  // no borrow: t >= 2p
+    FpR r;
+#pragma unroll
+    for (int i = 0; i < N; i++) r.v[i] = ge ? s[i] : t[i];
+    return r;
+  }
+  // a - b in (-2p, 2p); 2p added back when it borrowed -> [0, 2p)
+  friend PB_HD FpR operator-(const FpR& a, const FpR& b) {
+    uint32_t t[N];
+    t[0] = sub_cc(a.v[0], b.v[0]);
+#pragma unroll
+    for (int i = 1; i < N; i++) t[i] = subc_cc(a.v[i], b.v[i]);
+    const uint32_t m = subc(0u, 0u);  // 0xffffffff when a < b
+    FpR r;
+    r.v[0] = add_cc(t[0], MOD2(0) & m);
+#pragma unroll
+    for (int i = 1; i < N - 1; i++) r.v[i] = addc_cc(t[i], MOD2(i) & m);
+    r.v[N - 1] = addc(t[N - 1], MOD2(N - 1) & m);
+    return r;
+  }
+  PB_HD FpR neg() const { return zero() - *this; }  // 0 stays 0, else 2p - a
+  PB_HD FpR dbl() const { return *this + *this; }
+
+  // products: operands < 2p, result < 2p (no final subtraction)
+  friend PB_HD FpR operator*(const FpR& a, const FpR& b) { return from(Fp::mul<false>(a.raw(), b.raw())); }
+  PB_HD FpR sqr() const { return from(raw().sqr<false>()); }
+  // a*b + c*d and a*b - c*d with one Montgomery reduction (Field::mul2)
+  static PB_HD FpR mul2(const FpR& a, const FpR& b, const FpR& c, const FpR& d) {
+    return from(Fp::mul2<false>(a.raw(), b.raw(), c.raw(), d.raw()));
+  }
+  // -c enters the product as 2p - c, in (0, 2p]: no borrow to test, and an operand equal to 2p keeps every
+  // bound of Field::mul2 (the row peak is at most 5p * 2^32, the products sum to at most 8p^2 < p R).
+  static PB_HD FpR mul_sub(const FpR& a, const FpR& b, const FpR& c, const FpR& d) {
+    Fp nc;
+    nc.v[0] = sub_cc(MOD2(0), c.v[0]);
+#pragma unroll
+    for (int i = 1; i < N - 1; i++) nc.v[i] = subc_cc(MOD2(i), c.v[i]);
+    nc.v[N - 1] = subc(MOD2(N - 1), c.v[N - 1]);
+    return from(Fp::mul2<false>(a.raw(), b.raw(), nc, d.raw()));
+  }
+};
 
 }  // namespace pb

@@ -30,17 +30,18 @@ PB_D void ec_st_fp(uint4* q, const Fp& f) {
 }
 PB_D G1Xyzz ec_ld_xyzz(const uint4* p, size_t i) {
   G1Xyzz a;
-  a.x = ec_ld_fp(p + 12 * i);
-  a.y = ec_ld_fp(p + 12 * i + 3);
-  a.zz = ec_ld_fp(p + 12 * i + 6);
-  a.zzz = ec_ld_fp(p + 12 * i + 9);
+  a.x = FpR::from(ec_ld_fp(p + 12 * i));
+  a.y = FpR::from(ec_ld_fp(p + 12 * i + 3));
+  a.zz = FpR::from(ec_ld_fp(p + 12 * i + 6));
+  a.zzz = FpR::from(ec_ld_fp(p + 12 * i + 9));
   return a;
 }
-PB_D void ec_st_xyzz(uint4* p, size_t i, const G1Xyzz& a) {
-  ec_st_fp(p + 12 * i, a.x);
-  ec_st_fp(p + 12 * i + 3, a.y);
-  ec_st_fp(p + 12 * i + 6, a.zz);
-  ec_st_fp(p + 12 * i + 9, a.zzz);
+PB_D void ec_st_xyzz(uint4* p, size_t i, const G1Xyzz& a) {  // canonical, like every stored XYZZ point
+  const G1Xyzz c = a.canonical();
+  ec_st_fp(p + 12 * i, c.x.raw());
+  ec_st_fp(p + 12 * i + 3, c.y.raw());
+  ec_st_fp(p + 12 * i + 6, c.zz.raw());
+  ec_st_fp(p + 12 * i + 9, c.zzz.raw());
 }
 PB_D Fr ec_ld_fr(const uint4* p, size_t i) {
   const uint4 a = p[2 * i], b = p[2 * i + 1];

@@ -6,6 +6,11 @@
 // reference src/commitment_scheme/kzg10/commitment.rs:89-93), so we are free to pick the cheapest
 // coordinates: buckets are accumulated in XYZZ (x = X/ZZ, y = Y/ZZZ, ZZ^3 = ZZZ^2), where a mixed
 // addition of an affine base costs 8M + 2S and needs no field inversion.
+//
+// The XYZZ coordinates are FpR values (bigint.cuh: [0, 2p), products without the final subtraction).
+// Affine points stay canonical Fp and enter the formulas as they are.  Whatever leaves the formulas
+// for other code - affine normalisation, stored points - is made canonical on the way out
+// (xyzz_to_affine, G1Xyzz::canonical).
 #pragma once
 #include "bigint.cuh"
 
@@ -19,23 +24,28 @@ struct G1Affine {
 };
 
 struct G1Xyzz {
-  Fp x, y, zz, zzz;
+  FpR x, y, zz, zzz;
   static PB_HD G1Xyzz identity() {
     G1Xyzz r;
-    r.x = Fp::zero();
-    r.y = Fp::zero();
-    r.zz = Fp::zero();
-    r.zzz = Fp::zero();
+    r.x = FpR::zero();
+    r.y = FpR::zero();
+    r.zz = FpR::zero();
+    r.zzz = FpR::zero();
     return r;
   }
-  PB_HD bool is_inf() const { return zz.is_zero(); }
+  // The identity is the only point with zz = 0 mod p, and it always has the limbs zero, so a plain test
+  // suffices: identity() writes zeros, and every other zz is a product of factors that are nonzero mod p -
+  // one (from an affine point), zz * pp with pp = (u2 - u1)^2, where u2 - u1 = 0 mod p is caught by
+  // is_zero_mod_p and routed to the doubling or the identity, and zz * (2y)^2, where y = 0 mod p is caught
+  // the same way.  A product of nonzero residues is neither 0 nor p.
+  PB_HD bool is_inf() const { return zz.is_zero_limbs(); }
   static PB_HD G1Xyzz from_affine(const G1Affine& p) {
     G1Xyzz r;
     if (p.is_inf()) return identity();
-    r.x = p.x;
-    r.y = p.y;
-    r.zz = Fp::one();
-    r.zzz = Fp::one();
+    r.x = FpR::from(p.x);
+    r.y = FpR::from(p.y);
+    r.zz = FpR::one();
+    r.zzz = FpR::one();
     return r;
   }
   PB_HD G1Xyzz neg() const {
@@ -43,20 +53,29 @@ struct G1Xyzz {
     r.y = y.neg();
     return r;
   }
+  // every coordinate in [0, p): the form in which points are stored and handed to other code
+  PB_HD G1Xyzz canonical() const {
+    G1Xyzz r;
+    r.x = FpR::from(x.canonical());
+    r.y = FpR::from(y.canonical());
+    r.zz = FpR::from(zz.canonical());
+    r.zzz = FpR::from(zzz.canonical());
+    return r;
+  }
 };
 
 // 2*P for affine P (mdbl-2008-s-1).  P must not be the identity.
-PB_HD G1Xyzz xyzz_dbl_affine(const Fp& x1, const Fp& y1) {
+PB_HD G1Xyzz xyzz_dbl_affine(const FpR& x1, const FpR& y1) {
   G1Xyzz r;
-  if (y1.is_zero()) return G1Xyzz::identity();  // 2-torsion: cannot happen in the prime-order group
-  Fp u = y1.dbl();
-  Fp v = u.sqr();
-  Fp w = u * v;
-  Fp s = x1 * v;
-  Fp xx = x1.sqr();
-  Fp m = xx.dbl() + xx;
+  if (y1.is_zero_mod_p()) return G1Xyzz::identity();  // 2-torsion: cannot happen in the prime-order group
+  FpR u = y1.dbl();
+  FpR v = u.sqr();
+  FpR w = u * v;
+  FpR s = x1 * v;
+  FpR xx = x1.sqr();
+  FpR m = xx.dbl() + xx;
   r.x = m.sqr() - s.dbl();
-  r.y = Fp::mul_sub(m, s - r.x, w, y1);  // two products, one reduction
+  r.y = FpR::mul_sub(m, s - r.x, w, y1);  // two products, one reduction
   r.zz = v;
   r.zzz = w;
   return r;
@@ -65,16 +84,16 @@ PB_HD G1Xyzz xyzz_dbl_affine(const Fp& x1, const Fp& y1) {
 // 2*P in XYZZ (dbl-2008-s-1).
 PB_HD G1Xyzz xyzz_dbl(const G1Xyzz& p) {
   if (p.is_inf()) return p;
-  if (p.y.is_zero()) return G1Xyzz::identity();
+  if (p.y.is_zero_mod_p()) return G1Xyzz::identity();
   G1Xyzz r;
-  Fp u = p.y.dbl();
-  Fp v = u.sqr();
-  Fp w = u * v;
-  Fp s = p.x * v;
-  Fp xx = p.x.sqr();
-  Fp m = xx.dbl() + xx;
+  FpR u = p.y.dbl();
+  FpR v = u.sqr();
+  FpR w = u * v;
+  FpR s = p.x * v;
+  FpR xx = p.x.sqr();
+  FpR m = xx.dbl() + xx;
   r.x = m.sqr() - s.dbl();
-  r.y = Fp::mul_sub(m, s - r.x, w, p.y);
+  r.y = FpR::mul_sub(m, s - r.x, w, p.y);
   r.zz = v * p.zz;
   r.zzz = w * p.zzz;
   return r;
@@ -82,30 +101,31 @@ PB_HD G1Xyzz xyzz_dbl(const G1Xyzz& p) {
 
 // acc += (x2, +-y2) for an affine, non-identity point (madd-2008-s), all special cases handled:
 // acc = identity, acc == P (doubling), acc == -P (result is the identity).
-PB_HD void xyzz_madd(G1Xyzz& acc, const Fp& x2, const Fp& y2) {
+PB_HD void xyzz_madd(G1Xyzz& acc, const Fp& x2c, const Fp& y2c) {
+  const FpR x2 = FpR::from(x2c), y2 = FpR::from(y2c);
   if (acc.is_inf()) {
     acc.x = x2;
     acc.y = y2;
-    acc.zz = Fp::one();
-    acc.zzz = Fp::one();
+    acc.zz = FpR::one();
+    acc.zzz = FpR::one();
     return;
   }
-  Fp u2 = x2 * acc.zz;
-  Fp s2 = y2 * acc.zzz;
-  Fp p = u2 - acc.x;
-  Fp r = s2 - acc.y;
-  if (p.is_zero()) {
-    if (r.is_zero())
+  FpR u2 = x2 * acc.zz;
+  FpR s2 = y2 * acc.zzz;
+  FpR p = u2 - acc.x;
+  FpR r = s2 - acc.y;
+  if (p.is_zero_mod_p()) {
+    if (r.is_zero_mod_p())
       acc = xyzz_dbl_affine(x2, y2);
     else
       acc = G1Xyzz::identity();
     return;
   }
-  Fp pp = p.sqr();
-  Fp ppp = p * pp;
-  Fp q = acc.x * pp;
-  Fp x3 = r.sqr() - ppp - q.dbl();
-  Fp y3 = Fp::mul_sub(r, q - x3, acc.y, ppp);
+  FpR pp = p.sqr();
+  FpR ppp = p * pp;
+  FpR q = acc.x * pp;
+  FpR x3 = r.sqr() - ppp - q.dbl();
+  FpR y3 = FpR::mul_sub(r, q - x3, acc.y, ppp);
   acc.x = x3;
   acc.y = y3;
   acc.zz = acc.zz * pp;
@@ -119,24 +139,24 @@ PB_HD void xyzz_add(G1Xyzz& acc, const G1Xyzz& o) {
     acc = o;
     return;
   }
-  Fp u1 = acc.x * o.zz;
-  Fp u2 = o.x * acc.zz;
-  Fp s1 = acc.y * o.zzz;
-  Fp s2 = o.y * acc.zzz;
-  Fp p = u2 - u1;
-  Fp r = s2 - s1;
-  if (p.is_zero()) {
-    if (r.is_zero())
+  FpR u1 = acc.x * o.zz;
+  FpR u2 = o.x * acc.zz;
+  FpR s1 = acc.y * o.zzz;
+  FpR s2 = o.y * acc.zzz;
+  FpR p = u2 - u1;
+  FpR r = s2 - s1;
+  if (p.is_zero_mod_p()) {
+    if (r.is_zero_mod_p())
       acc = xyzz_dbl(acc);
     else
       acc = G1Xyzz::identity();
     return;
   }
-  Fp pp = p.sqr();
-  Fp ppp = p * pp;
-  Fp q = u1 * pp;
-  Fp x3 = r.sqr() - ppp - q.dbl();
-  Fp y3 = Fp::mul_sub(r, q - x3, s1, ppp);
+  FpR pp = p.sqr();
+  FpR ppp = p * pp;
+  FpR q = u1 * pp;
+  FpR x3 = r.sqr() - ppp - q.dbl();
+  FpR y3 = FpR::mul_sub(r, q - x3, s1, ppp);
   acc.x = x3;
   acc.y = y3;
   acc.zz = acc.zz * o.zz * pp;
@@ -164,7 +184,7 @@ PB_HD G1Xyzz xyzz_mul(const G1Xyzz& p, const uint32_t* k, int words) {
   return acc;
 }
 
-// Affine normalisation (one inversion): x = X/ZZ, y = Y/ZZZ.
+// Affine normalisation (one inversion): x = X/ZZ, y = Y/ZZZ, canonical.
 PB_HD G1Affine xyzz_to_affine(const G1Xyzz& p) {
   G1Affine r;
   if (p.is_inf()) {
@@ -172,11 +192,12 @@ PB_HD G1Affine xyzz_to_affine(const G1Xyzz& p) {
     r.y = Fp::zero();
     return r;
   }
-  Fp i = (p.zz * p.zzz).inv();
-  Fp izz = i * p.zzz;
-  Fp izzz = i * p.zz;
-  r.x = p.x * izz;
-  r.y = p.y * izzz;
+  const Fp zz = p.zz.canonical(), zzz = p.zzz.canonical();
+  Fp i = (zz * zzz).inv();
+  Fp izz = i * zzz;
+  Fp izzz = i * zz;
+  r.x = p.x.canonical() * izz;
+  r.y = p.y.canonical() * izzz;
   return r;
 }
 

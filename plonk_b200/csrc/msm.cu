@@ -81,18 +81,20 @@ PB_D void st_affine(uint4* p, size_t i, const G1Affine& a) {
   st_fp(p + 6 * i, a.x);
   st_fp(p + 6 * i + 3, a.y);
 }
-PB_D void st_xyzz(uint4* p, size_t i, const G1Xyzz& a) {  // 192 bytes
-  st_fp(p + 12 * i, a.x);
-  st_fp(p + 12 * i + 3, a.y);
-  st_fp(p + 12 * i + 6, a.zz);
-  st_fp(p + 12 * i + 9, a.zzz);
+// Stored XYZZ points are canonical (192 bytes): the host finish and the multi-GPU combine read the limbs.
+PB_D void st_xyzz(uint4* p, size_t i, const G1Xyzz& a) {
+  const G1Xyzz c = a.canonical();
+  st_fp(p + 12 * i, c.x.raw());
+  st_fp(p + 12 * i + 3, c.y.raw());
+  st_fp(p + 12 * i + 6, c.zz.raw());
+  st_fp(p + 12 * i + 9, c.zzz.raw());
 }
 PB_D G1Xyzz ld_xyzz(const uint4* p, size_t i) {
   G1Xyzz a;
-  a.x = ld_fp(p + 12 * i);
-  a.y = ld_fp(p + 12 * i + 3);
-  a.zz = ld_fp(p + 12 * i + 6);
-  a.zzz = ld_fp(p + 12 * i + 9);
+  a.x = FpR::from(ld_fp(p + 12 * i));
+  a.y = FpR::from(ld_fp(p + 12 * i + 3));
+  a.zz = FpR::from(ld_fp(p + 12 * i + 6));
+  a.zzz = FpR::from(ld_fp(p + 12 * i + 9));
   return a;
 }
 

@@ -70,8 +70,9 @@ PB_D G1Xyzz shfl_down_xyzz(const G1Xyzz& a, int d) {
 }
 PB_D G1Affine to_affine(const G1Xyzz& p) {
   if (p.is_inf()) return {Fp::zero(), Fp::zero()};
-  const Fp i = fp_inv_bingcd(p.zz * p.zzz);
-  return {p.x * (i * p.zzz), p.y * (i * p.zz)};
+  const Fp zz = p.zz.canonical(), zzz = p.zzz.canonical();
+  const Fp i = fp_inv_bingcd(zz * zzz);
+  return {p.x.canonical() * (i * zzz), p.y.canonical() * (i * zz)};
 }
 
 // Lane k of a warp multiplies term k of right_projective (proof.rs:300-455): the source of its point is a key
