@@ -19,6 +19,8 @@
  *   pb200_verifier_* / pb200_verify  Verifier / Verifier::verify (PlonkVersion::V3)
  *   pb200_verify_with_version        Verifier::verify_with_version (V1, V2 and V3)
  *                                    src/compiler/verifier.rs:32-263
+ *   pb200_batch_verify               one verdict for a batch with one pairing, after OpeningKey::batch_check
+ *                                    src/commitment_scheme/kzg10/key.rs:571-591, 650-707
  *
  * Data layout (identical to the reference's in-memory layout, SURVEY.md section 8):
  *   Fr  (BlsScalar)  4 x u64 little-endian limbs, Montgomery form R = 2^256        -> 32 bytes
@@ -272,6 +274,23 @@ int pb200_verify(const pb200_verifier_t* verifier, const uint8_t* proofs, size_t
  * pb200_plonk_version); the device work per proof is the same for all three versions. */
 int pb200_verify_with_version(const pb200_verifier_t* verifier, int version, const uint8_t* proofs, size_t n_proofs,
                               const uint64_t* pi_vals, size_t n_pi, int32_t* status);
+/* Batch verification: one verdict for n_proofs proofs under one version, at the cost of one pairing.  Arguments as
+ * pb200_verify_with_version.  Proof i's check e(L_i, [x]H) e(R_i, H) = 1, L_i = -(W_z + u_i W_zw), is folded into
+ * e(sum w_i L_i, [x]H) e(sum w_i R_i, H) = 1 with w_i = rho^i and rho drawn, as the reference's batch_challenge
+ * draws its challenge, from a merlin transcript over the whole batch: Transcript::new("dusk-plonk"), then
+ * "dom-sep" = "plonk-batch-verify-v1", "version" and "batch-len" (u64) and each proof's last challenge u_i under
+ * "batch-u", in batch order, and rho = challenge_scalar("batch-challenge").  A batch holding an invalid proof passes
+ * with probability at most (n_proofs - 1) / r.
+ * *verdict: PB200_OK when pb200_verify_with_version would give PB200_OK to every proof (up to that bound); otherwise
+ * PB200_ERR_POINT_MALFORMED when some proof fails Proof::from_bytes; otherwise PB200_ERR_VERIFY.  An empty batch is
+ * PB200_ERR_VERIFY, as batch_check rejects it.  The call fails with PB200_ERR_INVALID_ARG for a wrong n_pi
+ * (InconsistentPublicInputsLen), an unknown version or a NULL argument, and with PB200_ERR_CUDA on a device failure. */
+int pb200_batch_verify(const pb200_verifier_t* verifier, int version, const uint8_t* proofs, size_t n_proofs,
+                       const uint64_t* pi_vals, size_t n_pi, int32_t* verdict);
+/* Tests only: pb200_batch_verify that also returns the two folded points, sum w_i L_i then sum w_i R_i (96-byte raw
+ * layout each, zeros for the identity and when the verdict is decided before the pairing). */
+int pb200_selftest_batch_verify_points(const pb200_verifier_t* verifier, int version, const uint8_t* proofs, size_t n_proofs,
+                                       const uint64_t* pi_vals, size_t n_pi, int32_t* verdict, uint8_t* points_2x96);
 /* Tests only: the device pairing e(P_k, Q_k) for n G1 points (96-byte raw layout) and n compressed G2 points, as
  * Fp12 values of 576 bytes (c0.c0.c0, c0.c0.c1, c0.c1.c0, ..., c1.c2.c1; each Fp 6 x u64 Montgomery limbs). */
 int pb200_selftest_pairing(const uint64_t* g1_raw, const uint8_t* g2_compressed, size_t n, uint64_t* out_fp12);

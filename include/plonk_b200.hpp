@@ -437,9 +437,34 @@ class Verifier {
                                              pi.empty() ? nullptr : pi[0].data(), n_pi, st.data()));
     return st;
   }
+  // One verdict for the whole batch with one pairing (pb200_batch_verify): returns when every proof would pass
+  // verify_with_version (up to a chance of (n - 1) / r); throws PointMalformed when some proof fails
+  // Proof::from_bytes, otherwise ProofVerificationError, also for an empty batch.
+  void batch_verify(const std::vector<std::array<uint8_t, PROOF_SIZE>>& proofs, const std::vector<std::vector<BlsScalar>>& public_inputs,
+                    PlonkVersion version = PlonkVersion::V3) const {
+    if (proofs.size() != public_inputs.size()) throw Error(Error::InvalidArgument, "one public-input vector per proof");
+    const size_t n_pi = public_inputs.empty() ? pi_count() : public_inputs[0].size();
+    std::vector<BlsScalar> pi;
+    for (const auto& v : public_inputs) {
+      if (v.size() != n_pi) throw Error(Error::InvalidArgument, "every proof needs the same number of public inputs");
+      pi.insert(pi.end(), v.begin(), v.end());
+    }
+    int32_t verdict = PB200_OK;
+    check_verifier(pb200_batch_verify(h_, (int)version, proofs.empty() ? nullptr : proofs[0].data(), proofs.size(),
+                                      pi.empty() ? nullptr : pi[0].data(), n_pi, &verdict));
+    if (verdict == PB200_ERR_POINT_MALFORMED) throw Error(Error::PointMalformed, "InvalidData: malformed proof");
+    check_verifier(verdict);
+  }
 
  private:
   Verifier() = default;
+  // the public-input count, read back from Verifier::to_bytes (its fourth big-endian u64)
+  size_t pi_count() const {
+    const std::vector<uint8_t> b = to_bytes();
+    size_t n = 0;
+    for (int k = 24; k < 32; k++) n = (n << 8) | b[k];
+    return n;
+  }
   static void check_verifier(int rc) {
     if (rc == PB200_ERR_VERIFY) throw Error(Error::ProofVerificationError, "ProofVerificationError");
     if (rc == PB200_ERR_POINT_MALFORMED) throw Error(Error::PointMalformed, std::string("InvalidData: ") + pb200_last_error());

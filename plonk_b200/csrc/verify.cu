@@ -7,6 +7,11 @@
 // warp per proof (k_verify_msm), and runs the multi-Miller loop, the final exponentiation and the comparison with 1
 // with one thread per proof (k_verify_pairing).  The device work is the same for every version: V1 only gives the
 // four selector-opening terms zero scalars.
+//
+// Batch verification (pb200_batch_verify) gives one verdict for the whole batch with one pairing: the host draws
+// rho from the batch's u challenges (verify_scalars.h), k_batch_fold weighs each proof's terms by w_i = rho^i and
+// sums the verifier-key terms over the batch, k_batch_msm / k_batch_reduce form sum w_i L_i and sum w_i R_i, and
+// k_verify_pairing checks the pair.
 #include <algorithm>
 #include <mutex>
 #include <thread>
@@ -82,14 +87,11 @@ enum { P_A = 16, P_B, P_C, P_D, P_Z, P_TLOW, P_TMID, P_THIGH, P_TFOURTH, P_WZ, P
 __constant__ int c_term_point[32] = {0,  1,  2,  3,       4,      5,      7,       8,         9,    10, P_Z,   14, P_TLOW, P_TMID, P_THIGH, P_TFOURTH,
                                      P_A, P_B, P_C, P_D, 11, 12, 13, 6, 5, 1, 2, 15, P_WZ, P_WZW, -1, P_WZW};
 
-// One warp per proof.  scalars: [proof][32] canonical little-endian Fr; proof_comm: [proof][11] compressed
-// commitments; pts: their decoded points.  status: PB200_OK on entry or the host's verdict; a commitment that
-// decoded to zeros without being the identity's encoding is malformed.  out: [proof] -(W_z + u W_zw), right.
-__global__ void __launch_bounds__(128) k_verify_msm(const uint4* key_pts, const uint4* pts, const uint8_t* proof_comm,
-                                                    const uint4* scalars, size_t n, int* status, uint4* out) {
-  const size_t i = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int lane = threadIdx.x & 31;
-  if (i >= n) return;  // whole warps
+// Whether proof i has a malformed commitment, evaluated by a whole warp (lane k tests commitment k).  k_g1_decompress
+// leaves zeros for an encoding it rejects (not canonical, not on the curve or not torsion-free), so a commitment
+// that decoded to zeros without being the identity's encoding is malformed.  proof_comm: [proof][11] compressed
+// commitments; pts: their decoded points.
+PB_D bool warp_proof_malformed(const uint4* pts, const uint8_t* proof_comm, size_t i, int lane) {
   bool bad = false;
   if (lane < 11) {
     const uint4* q = pts + 6 * (i * 11 + lane);
@@ -101,7 +103,17 @@ __global__ void __launch_bounds__(128) k_verify_msm(const uint4* key_pts, const 
       bad = acc != 0;
     }
   }
-  if (__any_sync(0xffffffffu, bad)) {
+  return __any_sync(0xffffffffu, bad);
+}
+
+// One warp per proof.  scalars: [proof][32] canonical little-endian Fr; proof_comm, pts: as warp_proof_malformed.
+// status: PB200_OK on entry or the host's verdict.  out: [proof] -(W_z + u W_zw), right.
+__global__ void __launch_bounds__(128) k_verify_msm(const uint4* key_pts, const uint4* pts, const uint8_t* proof_comm,
+                                                    const uint4* scalars, size_t n, int* status, uint4* out) {
+  const size_t i = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (i >= n) return;  // whole warps
+  if (warp_proof_malformed(pts, proof_comm, i, lane)) {
     if (lane == 0) status[i] = PB200_ERR_POINT_MALFORMED;
     return;
   }
@@ -149,6 +161,146 @@ __global__ void __launch_bounds__(64) k_verify_pairing(const uint4* g1, const Li
   const LineCoeffs* l[2] = {lines, lines + PB_G2_LINES};
   const Fp12 f = final_exponentiation(miller_loop2(p, l));
   status[i] = f.is_one() ? PB200_OK : PB200_ERR_VERIFY;
+}
+
+// ---- batch verification -----------------------------------------------------------------------------------------
+// Proof i's check is e(L_i, [x]H) e(R_i, H) = 1 with L_i = -(W_z + u_i W_zw) and R_i = sum_k s_ik P_ik, the 31 terms
+// of k_verify_msm's lanes 0..30.  The batch's check is the same with L = sum w_i L_i and R = sum w_i R_i, formed as
+// two dense term lists: R has the 11 proof commitments of every proof (term 11 i + j is commitment j of proof i, so
+// its point is pts[11 i + j]) followed by the 16 key points, whose scalars are summed over the batch; L has W_z and
+// W_zw of every proof (terms 2 i and 2 i + 1) and is negated once at the end.
+constexpr int kBatchFoldWarps = 8;  // proofs per block of k_batch_fold
+
+PB_D Fr ld_fr(const uint4* q) {
+  Fr x;
+  const uint4 lo = q[0], hi = q[1];
+  x.v[0] = lo.x, x.v[1] = lo.y, x.v[2] = lo.z, x.v[3] = lo.w;
+  x.v[4] = hi.x, x.v[5] = hi.y, x.v[6] = hi.z, x.v[7] = hi.w;
+  return x;
+}
+PB_D void st_fr(uint4* q, const Fr& x) {
+  q[0] = make_uint4(x.v[0], x.v[1], x.v[2], x.v[3]);
+  q[1] = make_uint4(x.v[4], x.v[5], x.v[6], x.v[7]);
+}
+
+// One warp per proof, lane k on term k of k_verify_msm.  weights: [proof] w_i (Montgomery form, so that w_i times a
+// canonical scalar is canonical); status: the host's verdicts.  A proof that the host or the decoder rejected gets
+// weight 0 and sets flags (bit 0: malformed, bit 1: fails the check).  Writes the 11 n proof-term scalars of R
+// (r_scal) and the 2 n scalars of L (l_scal: w_i, w_i u_i), and per block the sums over its proofs of the 19
+// key-point lanes, merged into the 16 key points (key_part: [block][16]).
+__global__ void __launch_bounds__(32 * kBatchFoldWarps) k_batch_fold(const uint4* pts, const uint8_t* proof_comm, const uint4* scalars,
+                                                                    const uint4* weights, const int* status, size_t n, unsigned* flags,
+                                                                    uint4* r_scal, uint4* l_scal, uint4* key_part) {
+  __shared__ uint4 part[kBatchFoldWarps][32][2];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const size_t i = (size_t)blockIdx.x * kBatchFoldWarps + warp;
+  const int src = c_term_point[lane];
+  Fr prod = Fr::zero();
+  if (i < n) {  // whole warps
+    const bool bad = warp_proof_malformed(pts, proof_comm, i, lane);
+    const int st = bad ? PB200_ERR_POINT_MALFORMED : status[i];
+    if (lane == 0 && st != PB200_OK) atomicOr(flags, st == PB200_ERR_POINT_MALFORMED ? 1u : 2u);
+    const Fr w = st == PB200_OK ? ld_fr(weights + 2 * i) : Fr::zero();
+    prod = w * ld_fr(scalars + 2 * (i * PB_VERIFY_TERMS + lane));
+    if (lane == 31) {  // u: left's W_zw term
+      st_fr(l_scal + 2 * (2 * i), w.from_mont());
+      st_fr(l_scal + 2 * (2 * i + 1), prod);
+    } else if (src >= 16) {
+      st_fr(r_scal + 2 * (i * 11 + (src - 16)), prod);
+    }
+  }
+  st_fr(part[warp][lane], prod);
+  __syncthreads();
+  if (threadIdx.x < 16) {
+    Fr acc = Fr::zero();
+    for (int l = 0; l < 31; l++)
+      if (c_term_point[l] == (int)threadIdx.x)
+        for (int w = 0; w < kBatchFoldWarps; w++) acc = acc + ld_fr(part[w][l]);
+    st_fr(key_part + 2 * ((size_t)blockIdx.x * 16 + threadIdx.x), acc);
+  }
+}
+
+// Block k sums key point k's partial scalars over the n_blocks blocks of k_batch_fold into r_keys[k]; block 0 turns
+// the flags into the verdict (malformed before a failed check).
+__global__ void __launch_bounds__(256) k_batch_key_sums(const uint4* key_part, size_t n_blocks, const unsigned* flags, int* verdict,
+                                                        uint4* r_keys) {
+  __shared__ uint4 s[256][2];
+  Fr acc = Fr::zero();
+  for (size_t b = threadIdx.x; b < n_blocks; b += 256) acc = acc + ld_fr(key_part + 2 * (b * 16 + blockIdx.x));
+  st_fr(s[threadIdx.x], acc);
+  __syncthreads();
+  for (int d = 128; d >= 1; d >>= 1) {
+    if ((int)threadIdx.x < d) st_fr(s[threadIdx.x], ld_fr(s[threadIdx.x]) + ld_fr(s[threadIdx.x + d]));
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    st_fr(r_keys + 2 * blockIdx.x, ld_fr(s[0]));
+    if (blockIdx.x == 0) *verdict = (*flags & 1u) ? PB200_ERR_POINT_MALFORMED : (*flags & 2u) ? PB200_ERR_VERIFY : PB200_OK;
+  }
+}
+
+// One lane per term, 32 terms per warp: threads [0, r_pad) take R's n_r terms, threads [r_pad, r_pad + l_pad) take
+// L's n_l terms (both lists padded to whole warps with empty terms).  Per-lane double-and-add in XYZZ as in
+// k_verify_msm, then a warp sum; partial[warp] receives it.  Nothing runs once the verdict is a failure.
+__global__ void __launch_bounds__(128) k_batch_msm(const uint4* key_pts, const uint4* pts, const uint4* r_scal, size_t n_r,
+                                                   size_t r_pad, const uint4* l_scal, size_t n_l, size_t l_pad, const int* verdict,
+                                                   G1Xyzz* partial) {
+  const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= r_pad + l_pad || *verdict != PB200_OK) return;  // whole warps
+  const bool is_r = t < r_pad;
+  const size_t k = is_r ? t : t - r_pad;
+  G1Xyzz acc = G1Xyzz::identity();
+  if (k < (is_r ? n_r : n_l)) {
+    const size_t n_proof_terms = n_r - 16;
+    const G1Affine p = !is_r ? ld_aff(pts + 6 * ((k >> 1) * 11 + (P_WZ - 16) + (k & 1)))
+                       : k < n_proof_terms ? ld_aff(pts + 6 * k)
+                                           : ld_aff(key_pts + 6 * (k - n_proof_terms));
+    if (!p.is_inf()) {
+      const uint4* sp = (is_r ? r_scal : l_scal) + 2 * k;
+      const uint4 lo = sp[0], hi = sp[1];
+      const uint32_t s[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
+#pragma unroll 1
+      for (int w = 7; w >= 0; w--) {
+#pragma unroll 1
+        for (int b = 31; b >= 0; b--) {
+          acc = xyzz_dbl(acc);
+          if ((s[w] >> b) & 1u) xyzz_madd(acc, p.x, p.y);
+        }
+      }
+    }
+  }
+#pragma unroll 1
+  for (int d = 16; d >= 1; d >>= 1) {
+    const G1Xyzz o = shfl_down_xyzz(acc, d);
+    xyzz_add(acc, o);
+  }
+  if ((threadIdx.x & 31) == 0) partial[t >> 5] = acc;
+}
+
+// Block 0 sums R's r_warps warp partials, block 1 the l_warps after them and negates; out: L then R, 96-byte raw
+// affine each, the layout k_verify_pairing reads.
+__global__ void __launch_bounds__(256) k_batch_reduce(const G1Xyzz* partial, size_t r_warps, size_t l_warps, const int* verdict,
+                                                      uint4* out) {
+  __shared__ G1Xyzz s[8];
+  if (*verdict != PB200_OK) return;
+  const bool is_r = blockIdx.x == 0;
+  const G1Xyzz* p = is_r ? partial : partial + r_warps;
+  const size_t m = is_r ? r_warps : l_warps;
+  G1Xyzz acc = G1Xyzz::identity();
+#pragma unroll 1
+  for (size_t k = threadIdx.x; k < m; k += 256) xyzz_add(acc, p[k]);
+#pragma unroll 1
+  for (int d = 16; d >= 1; d >>= 1) {
+    const G1Xyzz o = shfl_down_xyzz(acc, d);
+    xyzz_add(acc, o);
+  }
+  if ((threadIdx.x & 31) == 0) s[threadIdx.x >> 5] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+#pragma unroll 1
+    for (int w = 1; w < 8; w++) xyzz_add(acc, s[w]);
+    st_aff(out + (is_r ? 6 : 0), to_affine(is_r ? acc : acc.neg()));
+  }
 }
 
 // Decodes `count` G2 points (96-byte encodings) and prepares the lines of each non-identity one.  ok[k]: 1 for a
@@ -286,6 +438,109 @@ int verifier_build(const uint8_t* label, size_t label_len, uint64_t vk_n, uint64
   return 0;
 }
 
+// The host stage of pb200_verify_with_version and pb200_batch_verify: per proof its commitments (comm), the 32
+// scalars of k_verify_msm (scal), the host's verdict (hstat) and, when us is given, its challenge u; spread over
+// threads for large batches.
+void replay(const pb200_verifier* V, int version, const uint8_t* proofs, size_t n_proofs, const uint64_t* pi_vals, size_t n_pi,
+            std::vector<uint64_t>& scal, std::vector<int>& hstat, std::vector<uint8_t>& comm, HFr* us) {
+  scal.assign(n_proofs * PB_VERIFY_TERMS * 4, 0);
+  hstat.assign(n_proofs, 0);
+  comm.assign(n_proofs * kProofEvalAt, 0);
+  auto work = [&](size_t lo, size_t hi) {
+    for (size_t i = lo; i < hi; i++) {
+      const uint8_t* pr = proofs + kProofBytes * i;
+      memcpy(comm.data() + kProofEvalAt * i, pr, kProofEvalAt);
+      hstat[i] = verify_scalars(V->key, version, pr, (const HFr*)(pi_vals + 4 * n_pi * i), scal.data() + (size_t)PB_VERIFY_TERMS * 4 * i,
+                                us ? us + i : nullptr);
+    }
+  };
+  const size_t n_thr = std::min<size_t>(std::max(1u, std::thread::hardware_concurrency()), std::min<size_t>(16, (n_proofs + 31) / 32));
+  if (n_thr <= 1) {
+    work(0, n_proofs);
+  } else {
+    std::vector<std::thread> th;
+    const size_t per = (n_proofs + n_thr - 1) / n_thr;
+    for (size_t t = 0; t < n_thr; t++) th.emplace_back(work, std::min(n_proofs, t * per), std::min(n_proofs, (t + 1) * per));
+    for (auto& x : th) x.join();
+  }
+}
+
+// pb200_batch_verify; points, when given, receives sum w_i L_i then sum w_i R_i (96-byte raw affine each; zeros when
+// the verdict is decided before the pairing).
+int batch_verify(const pb200_verifier_t* V, int version, const uint8_t* proofs, size_t n_proofs, const uint64_t* pi_vals, size_t n_pi,
+                 int32_t* verdict, uint8_t* points) {
+  PB_TRY(ensure_init());
+  if (!V || (!proofs && n_proofs) || (!pi_vals && n_pi && n_proofs) || !verdict) return fail(PB200_ERR_INVALID_ARG, "null argument");
+  if (version != PB200_PLONK_V1 && version != PB200_PLONK_V2 && version != PB200_PLONK_V3)
+    return fail(PB200_ERR_INVALID_ARG, "unknown PlonkVersion");
+  if (n_pi != V->pi_idx.size()) return fail(PB200_ERR_INVALID_ARG, "InconsistentPublicInputsLen");
+  if (points) memset(points, 0, 2 * 96);
+  if (!n_proofs) {  // batch_check rejects an empty batch (key.rs:667-669)
+    *verdict = PB200_ERR_VERIFY;
+    return 0;
+  }
+  PB_TRY(upload_pairing_consts());
+  std::vector<uint64_t> scal;
+  std::vector<int> hstat;
+  std::vector<uint8_t> comm;
+  std::vector<HFr> us(n_proofs);
+  replay(V, version, proofs, n_proofs, pi_vals, n_pi, scal, hstat, comm, us.data());
+  bool host_ok = true;
+  for (int h : hstat) {
+    if (h == PB200_ERR_POINT_MALFORMED) {
+      *verdict = PB200_ERR_POINT_MALFORMED;
+      return 0;
+    }
+    host_ok = host_ok && h == PB200_OK;
+  }
+  // rho is needed only when every proof passed the host stage; otherwise the verdict is a failure whatever the
+  // weights, and the device still looks for malformed commitments, which take precedence
+  const std::vector<HFr> w = host_ok ? batch_weights(batch_challenge(version, us.data(), n_proofs), n_proofs)
+                                     : std::vector<HFr>(n_proofs, HFr::zero());
+  const size_t n = n_proofs, fold_blocks = div_up(n, kBatchFoldWarps);
+  const size_t n_r = 11 * n + 16, r_pad = (n_r + 31) / 32 * 32, n_l = 2 * n, l_pad = (n_l + 31) / 32 * 32;
+  cudaStream_t st = thread_stream();
+  ScratchScope scope(nullptr, st);
+  uint8_t* d_comm;
+  uint4 *d_pts, *d_scal, *d_w, *d_rs, *d_ls, *d_keypart, *d_g1;
+  G1Xyzz* d_part;
+  unsigned *d_bad, *d_flags;
+  int *d_stat, *d_verdict;
+  PB_ALLOC(scope, d_comm, n * kProofEvalAt);
+  PB_ALLOC(scope, d_pts, n * 11 * 96);
+  PB_ALLOC(scope, d_scal, scal.size() * 8);
+  PB_ALLOC(scope, d_w, n * 32);
+  PB_ALLOC(scope, d_rs, n_r * 32);
+  PB_ALLOC(scope, d_ls, n_l * 32);
+  PB_ALLOC(scope, d_keypart, fold_blocks * 16 * 32);
+  PB_ALLOC(scope, d_part, (r_pad + l_pad) / 32 * sizeof(G1Xyzz));
+  PB_ALLOC(scope, d_g1, 2 * 96);
+  PB_ALLOC(scope, d_bad, 4);
+  PB_ALLOC(scope, d_flags, 4);
+  PB_ALLOC(scope, d_stat, n * sizeof(int));
+  PB_ALLOC(scope, d_verdict, sizeof(int));
+  static_assert(sizeof(HFr) == 32, "HFr: four little-endian words, the layout of a device Fr");
+  PB_CUDA(cudaMemcpyAsync(d_comm, comm.data(), n * kProofEvalAt, cudaMemcpyHostToDevice, st));
+  PB_CUDA(cudaMemcpyAsync(d_scal, scal.data(), scal.size() * 8, cudaMemcpyHostToDevice, st));
+  PB_CUDA(cudaMemcpyAsync(d_w, w.data(), n * 32, cudaMemcpyHostToDevice, st));
+  PB_CUDA(cudaMemcpyAsync(d_stat, hstat.data(), n * sizeof(int), cudaMemcpyHostToDevice, st));
+  PB_CUDA(cudaMemsetAsync(d_flags, 0, 4, st));
+  PB_CUDA(cudaMemsetAsync(d_g1, 0, 2 * 96, st));
+  g1_decompress_dev(d_comm, n * 11, d_pts, d_bad, st);
+  PB_LAUNCH(k_batch_fold, fold_blocks, 32 * kBatchFoldWarps, 0, st, d_pts, d_comm, d_scal, d_w, d_stat, n, d_flags, d_rs, d_ls, d_keypart);
+  PB_LAUNCH(k_batch_key_sums, 16, 256, 0, st, d_keypart, fold_blocks, d_flags, d_verdict, d_rs + 2 * 11 * n);
+  PB_LAUNCH(k_batch_msm, div_up(r_pad + l_pad, 128), 128, 0, st, V->d_points, d_pts, d_rs, n_r, r_pad, d_ls, n_l, l_pad, d_verdict, d_part);
+  PB_LAUNCH(k_batch_reduce, 2, 256, 0, st, d_part, r_pad / 32, l_pad / 32, d_verdict, d_g1);
+  PB_LAUNCH(k_verify_pairing, 1, 64, 0, st, d_g1, V->d_lines, 1, d_verdict);
+  PB_CUDA(cudaGetLastError());
+  int v = 0;
+  PB_CUDA(cudaMemcpyAsync(&v, d_verdict, sizeof(int), cudaMemcpyDeviceToHost, st));
+  if (points) PB_CUDA(cudaMemcpyAsync(points, d_g1, 2 * 96, cudaMemcpyDeviceToHost, st));
+  PB_CUDA(cudaStreamSynchronize(st));
+  *verdict = v;
+  return 0;
+}
+
 }  // namespace
 }  // namespace pb
 
@@ -378,26 +633,10 @@ int pb200_verify_with_version(const pb200_verifier_t* V, int version, const uint
   if (n_pi != V->pi_idx.size()) return fail(PB200_ERR_INVALID_ARG, "InconsistentPublicInputsLen");
   if (!n_proofs) return 0;
   PB_TRY(upload_pairing_consts());
-  // host: transcripts and scalars, spread over threads for large batches
-  std::vector<uint64_t> scal(n_proofs * PB_VERIFY_TERMS * 4);
-  std::vector<int> hstat(n_proofs);
-  std::vector<uint8_t> comm(n_proofs * kProofEvalAt);
-  auto work = [&](size_t lo, size_t hi) {
-    for (size_t i = lo; i < hi; i++) {
-      const uint8_t* pr = proofs + kProofBytes * i;
-      memcpy(comm.data() + kProofEvalAt * i, pr, kProofEvalAt);
-      hstat[i] = verify_scalars(V->key, version, pr,(const HFr*)(pi_vals + 4 * n_pi * i), scal.data() + (size_t)PB_VERIFY_TERMS * 4 * i);
-    }
-  };
-  const size_t n_thr = std::min<size_t>(std::max(1u, std::thread::hardware_concurrency()), std::min<size_t>(16, (n_proofs + 31) / 32));
-  if (n_thr <= 1) {
-    work(0, n_proofs);
-  } else {
-    std::vector<std::thread> th;
-    const size_t per = (n_proofs + n_thr - 1) / n_thr;
-    for (size_t t = 0; t < n_thr; t++) th.emplace_back(work, std::min(n_proofs, t * per), std::min(n_proofs, (t + 1) * per));
-    for (auto& x : th) x.join();
-  }
+  std::vector<uint64_t> scal;
+  std::vector<int> hstat;
+  std::vector<uint8_t> comm;
+  replay(V, version, proofs, n_proofs, pi_vals, n_pi, scal, hstat, comm, nullptr);
   // device: decoding, the two G1 points, the pairing check
   cudaStream_t st = thread_stream();
   ScratchScope scope(nullptr, st);
@@ -422,6 +661,17 @@ int pb200_verify_with_version(const pb200_verifier_t* V, int version, const uint
   PB_CUDA(cudaStreamSynchronize(st));
   for (size_t i = 0; i < n_proofs; i++) status[i] = hstat[i];
   return 0;
+}
+
+int pb200_batch_verify(const pb200_verifier_t* V, int version, const uint8_t* proofs, size_t n_proofs, const uint64_t* pi_vals,
+                       size_t n_pi, int32_t* verdict) {
+  return batch_verify(V, version, proofs, n_proofs, pi_vals, n_pi, verdict, nullptr);
+}
+
+int pb200_selftest_batch_verify_points(const pb200_verifier_t* V, int version, const uint8_t* proofs, size_t n_proofs,
+                                       const uint64_t* pi_vals, size_t n_pi, int32_t* verdict, uint8_t* points_2x96) {
+  if (!points_2x96) return fail(PB200_ERR_INVALID_ARG, "null argument");
+  return batch_verify(V, version, proofs, n_proofs, pi_vals, n_pi, verdict, points_2x96);
 }
 
 int pb200_selftest_pairing(const uint64_t* g1_raw, const uint8_t* g2_compressed, size_t n, uint64_t* out_fp12) {

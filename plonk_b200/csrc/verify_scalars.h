@@ -49,8 +49,10 @@ inline bool fr_canonical(const uint8_t* b, pbh::HFr* out) {  // BlsScalar::from_
 
 // Proof::verify (V2, V3) or Proof::verify_legacy (V1) up to the pairing: the transcript replay and the 32 scalars
 // of k_verify_msm (canonical form, in its term order).  version: a pb200_plonk_version.  Returns PB200_OK,
-// PB200_ERR_POINT_MALFORMED for a non-canonical evaluation or PB200_ERR_VERIFY.
-inline int verify_scalars(const VerifyKeyHost& K, int version, const uint8_t* proof, const pbh::HFr* pi, uint64_t* out) {
+// PB200_ERR_POINT_MALFORMED for a non-canonical evaluation or PB200_ERR_VERIFY.  u_out, when given, receives the
+// last challenge u (Montgomery form) of a proof that reaches it.
+inline int verify_scalars(const VerifyKeyHost& K, int version, const uint8_t* proof, const pbh::HFr* pi, uint64_t* out,
+                          pbh::HFr* u_out = nullptr) {
   using pbh::HFr;
   HFr e[N_EVAL];
   for (int k = 0; k < N_EVAL; k++)
@@ -64,6 +66,7 @@ inline int verify_scalars(const VerifyKeyHost& K, int version, const uint8_t* pr
   pbh::challenge_v(tr, e, c);
   pbh::challenge_u(tr, proof, c);
   const HFr &z = c.z, &v = c.v, &v_w = c.v_w, &u = c.u;
+  if (u_out) *u_out = u;
 
   const HFr one = HFr::one();
   const HFr z_n = z.pow_u64(K.n), z_h = z_n - one;
@@ -128,6 +131,31 @@ inline int verify_scalars(const VerifyKeyHost& K, int version, const uint8_t* pr
     memcpy(out + 4 * k, cn.v, 32);
   }
   return PB200_OK;
+}
+
+// The challenge rho of batch verification: w_i = rho^i weighs proof i's pairing check, and the batch passes iff
+// e(sum w_i L_i, [x]H) e(sum w_i R_i, H) = 1.  Drawn as the reference's batch_challenge (key.rs:571-591) draws its
+// challenge, from a transcript over the whole batch: the version, the length and each proof's u in batch order.  u
+// is the last Fiat-Shamir challenge of its proof, so it binds the key, the seed, the public inputs and every proof
+// byte, and rho is fixed only once the whole batch is.  us: Montgomery form; returns rho in Montgomery form.
+inline pbh::HFr batch_challenge(int version, const pbh::HFr* us, size_t n) {
+  pbh::Transcript t((const uint8_t*)"dusk-plonk", 10);
+  t.append_message("dom-sep", (const uint8_t*)"plonk-batch-verify-v1", 21);
+  t.append_u64("version", (uint64_t)version);
+  t.append_u64("batch-len", (uint64_t)n);
+  for (size_t i = 0; i < n; i++) t.append_scalar("batch-u", us[i]);
+  return t.challenge_scalar("batch-challenge");
+}
+
+// w_i = rho^i for i = 0 .. n-1 (Montgomery form).
+inline std::vector<pbh::HFr> batch_weights(const pbh::HFr& rho, size_t n) {
+  std::vector<pbh::HFr> w(n);
+  pbh::HFr acc = pbh::HFr::one();
+  for (size_t i = 0; i < n; i++) {
+    w[i] = acc;
+    acc = acc * rho;
+  }
+  return w;
 }
 
 }  // namespace pb

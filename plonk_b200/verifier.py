@@ -1,6 +1,5 @@
-"""Verifier (reference src/compiler/verifier.rs) on the GPU, through pb200_verifier_* and
-pb200_verify_with_version of include/plonk_b200.h.  Every PlonkVersion is verified on the device; V3 is the
-default."""
+"""Verifier (reference src/compiler/verifier.rs) on the GPU, through pb200_verifier_*, pb200_verify_with_version and
+pb200_batch_verify of include/plonk_b200.h.  Every PlonkVersion is verified on the device; V3 is the default."""
 from __future__ import annotations
 
 import ctypes
@@ -60,6 +59,29 @@ class Verifier:
         vals = b"".join(pi_vals)
         check(lib().pb200_verify_with_version(self._h, int(version), b"".join(proofs), len(proofs), vals or None, n_pi, status))
         return list(status[: len(proofs)])
+
+    def batch_verify(self, proofs: Sequence[bytes], pi_vals: Sequence[bytes], version: PlonkVersion = PlonkVersion.V3) -> None:
+        """One verdict for the whole batch at the cost of one pairing (pb200_batch_verify): returns when every proof
+        would pass verify_with_version (up to a chance of (len(proofs) - 1) / r), raises PointMalformed when some
+        proof fails Proof::from_bytes, otherwise ProofVerificationError, also for an empty batch; ValueError for
+        inconsistent public inputs or an unknown version."""
+        assert len(proofs) == len(pi_vals) and all(len(p) == PROOF_BYTES for p in proofs)
+        n_pi = len(pi_vals[0]) // 32 if pi_vals else self.n_pi
+        if any(len(v) != 32 * n_pi for v in pi_vals):
+            raise ValueError("every proof needs the same number of public inputs")
+        verdict = ctypes.c_int32()
+        vals = b"".join(pi_vals)
+        try:
+            check(lib().pb200_batch_verify(self._h, int(version), b"".join(proofs) or None, len(proofs), vals or None, n_pi,
+                                           ctypes.byref(verdict)))
+        except Pb200Error as e:
+            if e.code == PB200_ERR_INVALID_ARG:
+                raise ValueError(str(e)) from e
+            raise
+        if verdict.value == PB200_ERR_VERIFY:
+            raise ProofVerificationError("ProofVerificationError")
+        if verdict.value == PB200_ERR_POINT_MALFORMED:
+            raise PointMalformed("InvalidData")
 
     def verify(self, proof: bytes, pi_vals: bytes) -> None:
         """Verifier::verify: returns on success, raises ProofVerificationError, PointMalformed or ValueError."""
