@@ -12,8 +12,12 @@
  *                                    src/commitment_scheme/kzg10/key.rs:36-41
  *   pb200_g1_compress                G1Affine::to_bytes as used by Commitment::to_bytes
  *                                    src/commitment_scheme/kzg10/commitment.rs:95-101
+ *   pb200_g1_compress_batch          CommitKey::to_var_bytes            src/commitment_scheme/kzg10/key.rs:303-308
+ *   pb200_commit_key_to_raw_var_bytes CommitKey::to_raw_var_bytes       src/commitment_scheme/kzg10/key.rs:215-229
  *   pb200_prover_* / pb200_prove     Prover::new / Prover::prove (PlonkVersion::V3)
  *                                    src/compiler/prover.rs:53-115, 415-761
+ *   pb200_prover_from_bytes / _to_bytes  Prover::try_from_bytes / Prover::to_bytes
+ *                                    src/compiler/prover.rs:212-350
  *   pb200_prove_with_version         Prover::prove_with_version (V2 and V3; V1 is refused as the reference does)
  *                                    src/compiler/prover.rs:364-413
  *   pb200_verifier_* / pb200_verify  Verifier / Verifier::verify (PlonkVersion::V3)
@@ -175,8 +179,20 @@ int pb200_g1_decompress(const uint8_t* compressed, size_t n_points, int check_su
 #define PB200_OPENING_KEY_BYTES 240
 int pb200_raw_commit_key_points(const uint8_t* bytes, size_t len, int checked, size_t* n_points);
 int pb200_commit_key_from_raw_var_bytes(const uint8_t* bytes, size_t len, int checked, uint8_t* out_raw);
+/* CommitKey::to_raw_var_bytes (key.rs:215-229), the writer of the format above: the u64 little-endian count, then
+ * PB200_G1_RAW_SIZE bytes per point - the 96 raw bytes and a zero flag; the identity (96 zero bytes here) is written
+ * as the reference's G1Affine::identity(): x = 0, y = Montgomery one, flag 1.  Host only, no device needed.
+ * PublicParameters::to_raw_var_bytes (srs.rs:114-119) is this behind the 240 bytes of OpeningKey::to_bytes.
+ * *len always receives 8 + n_points x 97; out = NULL writes nothing else; cap < *len is PB200_ERR_INVALID_ARG and
+ * `out` is left untouched. */
+int pb200_commit_key_to_raw_var_bytes(const uint8_t* raw_points, size_t n_points, uint8_t* out, size_t cap, size_t* len);
 /* 48-byte compressed encoding of one affine point given in the 96-byte raw layout. */
 int pb200_g1_compress(const uint64_t* affine_raw, uint8_t out48[48]);
+/* CommitKey::to_var_bytes (key.rs:303-308; PublicParameters::to_var_bytes, srs.rs:149-153, is the same behind the
+ * opening key): n_points x 96-byte raw points -> n_points x 48 bytes, G1Affine::to_bytes per point, byte for byte
+ * what pb200_g1_compress gives.  The inverse of pb200_g1_decompress; runs on the GPU, one thread per point.
+ * n_points = 0 is PB200_OK. */
+int pb200_g1_compress_batch(const uint8_t* raw_points, size_t n_points, uint8_t* out_48);
 /* out = a + b for two points in the 96-byte raw layout (host-side helper for multi-GPU reduction). */
 int pb200_g1_add_affine(const uint64_t* a_raw, const uint64_t* b_raw, uint64_t* out_raw);
 
@@ -197,7 +213,8 @@ int pb200_prover_new(const uint8_t* label, size_t label_len, size_t n_constraint
  * ProverKey::to_var_bytes (src/proof_system/widget.rs:347-445: n, the byte size of one Evaluations, then for
  * each of the 15 polynomials its coefficient count, canonical 32-byte coefficients and its 8n coset
  * evaluations, then the linear and vanishing-polynomial evaluations), the commit key in the raw format above
- * and VerifierKey::to_bytes (widget.rs:84-111: n and 15 compressed commitments).  The polynomials go to HBM in
+ * and VerifierKey::to_bytes (widget.rs:84-111: n - the constraint count, compiler.rs:278-279, which try_from_bytes
+ * compares with nothing and neither does this loader - and 15 compressed commitments).  The polynomials go to HBM in
  * coefficient form and the commitments are taken as stored, so none of the 15 iNTTs / 15 MSMs of preprocessing
  * runs; the 8n evaluations are recomputed by 16 coset NTTs on the device (faster than moving 17 x 8n scalars
  * over PCIe), so the serialized ones are skipped, not read.  Errors as the reference: too short ->
@@ -207,6 +224,17 @@ int pb200_prover_new(const uint8_t* label, size_t label_len, size_t n_constraint
  * the wires from that composer), so `wires` (4 x constraints witness indices) and n_witnesses come with it. */
 int pb200_prover_from_bytes(const uint8_t* bytes, size_t len, const uint32_t* wires, size_t n_witnesses,
                             pb200_prover_t** out);
+/* Prover::to_bytes (prover.rs:238-263) and Prover::serialized_size (:233-235): the layout pb200_prover_from_bytes
+ * reads, for a prover made by pb200_prover_new or by pb200_prover_from_bytes.  Each polynomial is written with its
+ * trailing zero coefficients dropped (Polynomial::from_coefficients_vec, polynomial.rs:79-93; a selector the circuit
+ * never uses has length 0), the commit key is the trimmed one the prover holds (pb200_srs_len points), and
+ * VerifierKey::n is the constraint count (compiler.rs:278-279).  The scalars leave HBM in chunks, converted to
+ * canonical form on the device; no second copy of the key is made there.  The call reads only what the prover never
+ * changes, so it may run beside proofs on the same prover; it uses the calling thread's pb200 stream.
+ * *len always receives the size; out = NULL writes nothing else; cap < *len is PB200_ERR_INVALID_ARG and `out` is
+ * left untouched.  The reference's Prover::try_from_bytes has not been run on these bytes (the raw point record is
+ * restated, not pinned - see PB200_G1_RAW_SIZE). */
+int pb200_prover_to_bytes(const pb200_prover_t* prover, uint8_t* out, size_t cap, size_t* len);
 void pb200_prover_free(pb200_prover_t* prover);
 /* 15 compressed commitments (verifier-key material) in the order of `selectors` then s_sigma_1..4. */
 int pb200_prover_commitments(const pb200_prover_t* prover, uint8_t* out_15x48);

@@ -4,9 +4,11 @@
 // caller links against, with the reference's names, argument meaning and error behaviour:
 //
 //   plonk_b200::EvaluationDomain   src/fft/domain.rs:35-232      new / fft / ifft / coset_fft / coset_ifft
-//   plonk_b200::CommitKey          src/commitment_scheme/kzg10/key.rs:36-41, 362-388   commit, max_degree
+//   plonk_b200::CommitKey          src/commitment_scheme/kzg10/key.rs:36-41, 215-308, 362-388   commit, max_degree,
+//                                                                                      to_var_bytes, to_raw_var_bytes
 //   plonk_b200::Commitment         src/commitment_scheme/kzg10/commitment.rs:77-106    to_bytes (48 B)
-//   plonk_b200::Prover             src/compiler/prover.rs:53-115, 352-413              prove, prove_with_version
+//   plonk_b200::Prover             src/compiler/prover.rs:53-115, 212-413              prove, prove_with_version, to_bytes,
+//                                                                                      serialized_size, try_from_bytes
 //   plonk_b200::Verifier           src/compiler/verifier.rs:32-263                     verify, verify_with_version, to_bytes,
 //                                                                                      try_from_bytes
 //   plonk_b200::PlonkVersion       src/compiler.rs:22-42
@@ -101,7 +103,24 @@ struct Commitment {
 class CommitKey {
  public:
   // powers_of_g as 96-byte raw points (CommitKey::to_raw_var_bytes without length prefix / flags)
-  CommitKey(const uint8_t* raw_points, size_t n_points) : n_(n_points) { check(pb200_srs_upload(raw_points, n_points, &h_)); }
+  CommitKey(const uint8_t* raw_points, size_t n_points) : n_(n_points), raw_(raw_points, raw_points + 96 * n_points) {
+    check(pb200_srs_upload(raw_points, n_points, &h_));
+  }
+  // CommitKey::to_var_bytes (key.rs:303-308): G1Affine::to_bytes per point, encoded on the GPU; what
+  // CommitKey::from_slice reads
+  std::vector<uint8_t> to_var_bytes() const {
+    std::vector<uint8_t> out(48 * n_);
+    check(pb200_g1_compress_batch(raw_.data(), n_, out.data()));
+    return out;
+  }
+  // CommitKey::to_raw_var_bytes (key.rs:215-229): what from_raw_var_bytes and from_slice_unchecked read
+  std::vector<uint8_t> to_raw_var_bytes() const {
+    size_t n = 0;
+    check(pb200_commit_key_to_raw_var_bytes(raw_.data(), n_, nullptr, 0, &n));
+    std::vector<uint8_t> out(n);
+    check(pb200_commit_key_to_raw_var_bytes(raw_.data(), n_, out.data(), out.size(), &n));
+    return out;
+  }
   // CommitKey::from_raw_var_bytes (key.rs:258-298: every point validated, on the GPU) and
   // CommitKey::from_slice_unchecked (key.rs:242-256: trusted bytes) for CommitKey::to_raw_var_bytes
   static std::unique_ptr<CommitKey> from_raw_var_bytes(const uint8_t* bytes, size_t len) { return from_raw(bytes, len, 1); }
@@ -124,6 +143,7 @@ class CommitKey {
  private:
   pb200_srs_t* h_ = nullptr;
   size_t n_;
+  std::vector<uint8_t> raw_;  // the points the key was made from (96 bytes each), kept for the two writers
   static std::unique_ptr<CommitKey> from_raw(const uint8_t* bytes, size_t len, int checked) {
     size_t n = 0;
     check(pb200_raw_commit_key_points(bytes, len, checked, &n));
@@ -346,6 +366,18 @@ class Prover {
     p->n_witnesses_ = n_witnesses;
     check(pb200_prover_from_bytes(bytes, len, wires.data(), n_witnesses, &p->h_));
     return p;
+  }
+  // Prover::serialized_size (prover.rs:233-235) and Prover::to_bytes (:238-263): the bytes try_from_bytes reads
+  size_t serialized_size() const {
+    size_t n = 0;
+    check(pb200_prover_to_bytes(h_, nullptr, 0, &n));
+    return n;
+  }
+  std::vector<uint8_t> to_bytes() const {
+    size_t n = serialized_size();
+    std::vector<uint8_t> out(n);
+    check(pb200_prover_to_bytes(h_, out.data(), out.size(), &n));
+    return out;
   }
   ~Prover() { pb200_prover_free(h_); }
   Prover(const Prover&) = delete;

@@ -40,7 +40,8 @@ EXPORTS = [
     "pb200_ntt", "pb200_ntt_dev",
     "pb200_srs_upload", "pb200_srs_upload_window", "pb200_msm_window_for", "pb200_srs_window", "pb200_srs_free", "pb200_srs_len",
     "pb200_msm_g1", "pb200_msm_g1_dev", "pb200_msm_g1_range", "pb200_msm_g1_allgather", "pb200_msm_g1_allgather_dev", "pb200_msm_combine_parts",
-    "pb200_g1_compress", "pb200_g1_decompress", "pb200_raw_commit_key_points", "pb200_commit_key_from_raw_var_bytes", "pb200_g1_add_affine", "pb200_srs_setup_from_secret", "pb200_g1_lagrange_key",
+    "pb200_g1_compress", "pb200_g1_compress_batch", "pb200_g1_decompress", "pb200_raw_commit_key_points", "pb200_commit_key_from_raw_var_bytes",
+    "pb200_commit_key_to_raw_var_bytes", "pb200_prover_to_bytes", "pb200_g1_add_affine", "pb200_srs_setup_from_secret", "pb200_g1_lagrange_key",
     "pb200_profile_enable", "pb200_throughput_mode", "pb200_profile_read", "pb200_profile_read_sparse",
     "pb200_prover_new", "pb200_prover_from_bytes", "pb200_prover_free", "pb200_prover_commitments", "pb200_prove", "pb200_prove_dev",
     "pb200_prove_with_version", "pb200_prove_dev_with_version",
@@ -110,6 +111,9 @@ def lib() -> ctypes.CDLL:
         L.pb200_raw_commit_key_points.argtypes = [c.c_void_p, c.c_size_t, c.c_int, c.POINTER(c.c_size_t)]
         L.pb200_commit_key_from_raw_var_bytes.argtypes = [c.c_void_p, c.c_size_t, c.c_int, c.c_void_p]
         L.pb200_prover_from_bytes.argtypes = [c.c_void_p, c.c_size_t, c.c_void_p, c.c_size_t, c.POINTER(c.c_void_p)]
+        L.pb200_prover_to_bytes.argtypes = [c.c_void_p, c.c_void_p, c.c_size_t, c.POINTER(c.c_size_t)]
+        L.pb200_g1_compress_batch.argtypes = [c.c_void_p, c.c_size_t, c.c_void_p]
+        L.pb200_commit_key_to_raw_var_bytes.argtypes = [c.c_void_p, c.c_size_t, c.c_void_p, c.c_size_t, c.POINTER(c.c_size_t)]
         L.pb200_g1_add_affine.argtypes = [c.c_void_p, c.c_void_p, c.c_void_p]
         L.pb200_prover_new.argtypes = [c.c_void_p, c.c_size_t, c.c_size_t, c.c_void_p, c.c_void_p, c.c_size_t, c.c_void_p, c.c_size_t, c.POINTER(c.c_void_p)]
         L.pb200_prover_free.argtypes = [c.c_void_p]

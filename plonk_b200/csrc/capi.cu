@@ -115,6 +115,7 @@ int msm_window_for(size_t n_points);
 int srs_setup(const uint64_t* x_mont, const uint64_t* g_scalar_mont, size_t n, uint8_t* out_raw);
 int g1_decompress(const uint8_t* in, size_t n, int check_subgroup, uint8_t* out_raw);
 int g1_check_raw(const uint8_t* raw, size_t n);
+int g1_compress_batch(const uint8_t* raw, size_t n, uint8_t* out_48);
 int raw_commit_key_parse(const uint8_t* bytes, size_t len, int checked, size_t* n_points, uint8_t* out_raw);
 extern std::atomic<int> g_prof_on;
 extern std::atomic<uint64_t> g_prof_acc_ns, g_prof_acc_adds, g_prof_acc_launches, g_prof_acc_points;
@@ -149,6 +150,17 @@ int raw_commit_key_parse(const uint8_t* bytes, size_t len, int checked, size_t* 
         memcpy(out_raw + 96 * i, rec, 96);
     }
   return 0;
+}
+
+// One record of CommitKey::to_raw_var_bytes (G1Affine::to_raw_bytes): the 96 raw bytes and a zero flag; this
+// library's identity (96 zero bytes) becomes the reference's G1Affine::identity(): x = 0, y = 1 (Montgomery form),
+// flag 1 - what raw_commit_key_parse maps back.
+void raw_commit_key_record(const uint8_t* raw96, uint8_t* rec97) {
+  bool zero = true;
+  for (int i = 0; i < 96 && zero; i++) zero = raw96[i] == 0;
+  memcpy(rec97, raw96, 96);
+  if (zero) memcpy(rec97 + 48, pbh::kFpMod.r1, 48);
+  rec97[96] = zero ? 1 : 0;
 }
 }  // namespace pb
 
@@ -374,6 +386,24 @@ int pb200_commit_key_from_raw_var_bytes(const uint8_t* bytes, size_t len, int ch
     PB_TRY(g1_check_raw(out_raw, n));
   }
   return 0;
+}
+
+int pb200_commit_key_to_raw_var_bytes(const uint8_t* raw_points, size_t n_points, uint8_t* out, size_t cap, size_t* len) {
+  if (!len || (!raw_points && n_points)) return fail(PB200_ERR_INVALID_ARG, "null argument");
+  const size_t total = 8 + n_points * PB200_G1_RAW_SIZE;
+  *len = total;
+  if (!out) return 0;
+  if (cap < total) return fail(PB200_ERR_INVALID_ARG, "output buffer too small");
+  for (int i = 0; i < 8; i++) out[i] = (uint8_t)((uint64_t)n_points >> (8 * i));
+  for (size_t i = 0; i < n_points; i++) raw_commit_key_record(raw_points + 96 * i, out + 8 + i * PB200_G1_RAW_SIZE);
+  return 0;
+}
+
+int pb200_g1_compress_batch(const uint8_t* raw_points, size_t n_points, uint8_t* out_48) {
+  PB_TRY(ensure_init());
+  if (!n_points) return 0;
+  if (!raw_points || !out_48) return fail(PB200_ERR_INVALID_ARG, "null argument");
+  return g1_compress_batch(raw_points, n_points, out_48);
 }
 
 int pb200_srs_setup_from_secret(const uint64_t* x, const uint64_t* g_scalar, size_t n_points, uint8_t* out_raw) {

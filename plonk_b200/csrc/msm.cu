@@ -251,6 +251,39 @@ __global__ void __launch_bounds__(64) k_g1_check_raw(const uint4* pts, size_t n,
   if (!ok) atomicMin(bad, (unsigned)i);
 }
 
+// G1Affine::to_bytes for a whole commit key (CommitKey::to_var_bytes, key.rs:303-308), the inverse of
+// k_g1_decompress and the device twin of pbh::g1_compress_raw: big-endian canonical x with bit 7 set, bit 5 when
+// y > (p - 1) / 2; the identity is 0xc0 and zeros.  One thread per point, 48 bytes out as three 128-bit stores.
+__global__ void __launch_bounds__(128) k_g1_compress(const uint4* __restrict__ pts, size_t n, uint4* __restrict__ out) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const G1Affine p = ld_affine(pts, i);
+  Fp x = Fp::zero();
+  uint32_t flags = 0xc0000000u;
+  if (!p.is_inf()) {
+    x = p.x.from_mont();
+    // y is "the larger root" iff y > p - y as integers
+    const Fp yc = p.y.from_mont(), nc = p.y.neg().from_mont();
+    bool larger = false;
+#pragma unroll
+    for (int k = 11; k >= 0; k--) {
+      if (yc.v[k] != nc.v[k]) {
+        larger = yc.v[k] > nc.v[k];
+        break;
+      }
+    }
+    flags = 0x80000000u | (larger ? 0x20000000u : 0u);
+  }
+  x.v[11] |= flags;
+  uint32_t be[12];  // byte 4k..4k+3 of the encoding = limb 11-k, most significant byte first
+#pragma unroll
+  for (int k = 0; k < 12; k++) be[k] = __byte_perm(x.v[11 - k], 0u, 0x0123);
+  uint4* o = out + 3 * i;
+  o[0] = make_uint4(be[0], be[1], be[2], be[3]);
+  o[1] = make_uint4(be[4], be[5], be[6], be[7]);
+  o[2] = make_uint4(be[8], be[9], be[10], be[11]);
+}
+
 // Signed-digit recoding + bucket histogram.  ebkt/epos are [batch][W][n].
 __global__ void k_msm_digits(const uint4* scalars, size_t n, size_t stride, int c, int W, unsigned nb,
                              unsigned* counts, unsigned* ebkt, unsigned* epos) {
@@ -1681,6 +1714,21 @@ int g1_check_raw(const uint8_t* raw, size_t n) {
     snprintf(msg, sizeof msg, "point %u", bad);
     return fail(PB200_ERR_POINT_MALFORMED, "commit-key point not on the curve or not in the prime-order subgroup (PointMalformed)", msg);
   }
+  return 0;
+}
+
+// n raw points (host) -> n x 48 compressed bytes (host): CommitKey::to_var_bytes
+int g1_compress_batch(const uint8_t* raw, size_t n, uint8_t* out_48) {
+  cudaStream_t st = thread_stream();
+  ScratchScope scope(nullptr, st);
+  uint4 *d_in = nullptr, *d_out = nullptr;
+  PB_ALLOC(scope, d_in, n * 96);
+  PB_ALLOC(scope, d_out, n * 48);
+  PB_CUDA(cudaMemcpyAsync(d_in, raw, n * 96, cudaMemcpyHostToDevice, st));
+  PB_LAUNCH(k_g1_compress, div_up(n, 128), 128, 0, st, (const uint4*)d_in, n, d_out);
+  PB_CUDA(cudaGetLastError());
+  PB_CUDA(cudaMemcpyAsync(out_48, d_out, n * 48, cudaMemcpyDeviceToHost, st));
+  PB_CUDA(cudaStreamSynchronize(st));
   return 0;
 }
 

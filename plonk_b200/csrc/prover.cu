@@ -48,6 +48,7 @@ extern thread_local int t_msm_wide_heavy_chunks;
 static std::atomic<int> g_force_throughput{0};
 int g1_check_raw(const uint8_t* raw, size_t n);
 int raw_commit_key_parse(const uint8_t* bytes, size_t len, int checked, size_t* n_points, uint8_t* out_raw);
+void raw_commit_key_record(const uint8_t* raw96, uint8_t* rec97);
 int lagrange_key_dev(const uint4* d_in, int log_n, uint4* d_out, cudaStream_t st);
 int get_twiddles(int logm, bool inverse, cudaStream_t st, const uint4** out);
 int fill_powers(uint4* out, size_t n, const Fr& base, const Fr& scale, cudaStream_t st);
@@ -139,6 +140,35 @@ __global__ void k_fr_from_canonical(uint4* p, size_t n_elems, unsigned* flag) {
   }
   if (!lt) atomicOr(flag, 1u);
   stg_fr(p, i, x.to_mont());
+}
+
+// BlsScalar::to_bytes for a whole array, the inverse of k_fr_from_canonical: one Montgomery product by 1 per
+// scalar; the output limbs are little-endian, i.e. the 32 bytes the reference writes.
+__global__ void k_fr_to_canonical(const uint4* __restrict__ in, size_t n_elems, uint4* __restrict__ out) {
+  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n_elems) stg_fr(out, i, ldg_fr(in, i).from_mont());
+}
+
+// Polynomial::from_coefficients_vec drops trailing zero coefficients (polynomial.rs:79-93): len[row] = index of
+// the row's last non-zero coefficient + 1, 0 for an all-zero row.  polys is [gridDim.y][n], len starts at zero;
+// one atomicMax per block and row.
+__global__ void k_poly_trim_len(const uint4* __restrict__ polys, size_t n, unsigned* len) {
+  const unsigned row = blockIdx.y;
+  const uint4* p = polys + 2 * (size_t)row * n;
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  unsigned m = 0;
+  if (i < n) {
+    const uint4 a = __ldg(p + 2 * i), b = __ldg(p + 2 * i + 1);
+    if (a.x | a.y | a.z | a.w | b.x | b.y | b.z | b.w) m = (unsigned)i + 1;
+  }
+  m = __reduce_max_sync(0xffffffffu, m);
+  __shared__ unsigned warp_max[32];
+  if ((threadIdx.x & 31) == 0) warp_max[threadIdx.x >> 5] = m;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (unsigned w = 1; w < (blockDim.x + 31) / 32; w++) m = max(m, warp_max[w]);
+    if (m) atomicMax(len + row, m);
+  }
 }
 
 __global__ void k_zero(uint4* p, size_t n_elems) {
@@ -873,7 +903,8 @@ int prover_from_bytes(const uint8_t* bytes, size_t len, const uint32_t* wires, s
   }
   // VerifierKey::to_bytes (widget.rs:84-111)
   if (vk_len < 8 + 15 * 48) return fail(short_rc, "NotEnoughBytes: verifier key");
-  if (le64(vk) != size) return fail(bad_rc, "InvalidData: verifier key domain differs from the prover's size");
+  // VerifierKey::n is the circuit's constraint count (compiler.rs:278-279) and try_from_bytes compares it with
+  // nothing (prover.rs:331-348); the transcript takes the prover's own constraint count instead (prove_dev)
   for (int i = 0; i < N_POLY; i++) memcpy(key.comm[kKeyFileOrder[i]], vk + 8 + 48 * i, 48);
   // CommitKey::from_raw_var_bytes: validated points
   size_t n_pts = 0;
@@ -889,6 +920,197 @@ int prover_from_bytes(const uint8_t* bytes, size_t len, const uint32_t* wires, s
   }
   *out = P;
   return 0;
+}
+
+// Moves key material from HBM into the caller's (pageable) buffer without a second copy of the key on the device:
+// chunks of kChunk bytes go through two device scratch blocks and the calling thread's two pinned buffers, so the
+// device converts and copies chunk k + 1 while the host moves chunk k from pinned memory to its place in `out`.
+struct KeyStreamer {
+  static constexpr size_t kChunk = (size_t)8 << 20;
+  cudaStream_t st;
+  uint4* d_buf[2] = {nullptr, nullptr};
+  uint8_t* h_buf[2] = {nullptr, nullptr};
+  cudaEvent_t ev[2] = {nullptr, nullptr};
+  struct Pending {
+    uint8_t* dst = nullptr;
+    size_t count = 0;
+    bool points = false;
+  } pend[2];
+  unsigned issued = 0;
+
+  explicit KeyStreamer(cudaStream_t s) : st(s) {}
+  ~KeyStreamer() {
+    for (int b = 0; b < 2; b++) {
+      if (pend[b].count) cudaEventSynchronize(ev[b]);  // an error path: the pinned buffers outlive this call
+      if (d_buf[b]) cudaFreeAsync(d_buf[b], st);
+      if (ev[b]) cudaEventDestroy(ev[b]);
+    }
+  }
+  KeyStreamer(const KeyStreamer&) = delete;
+  KeyStreamer& operator=(const KeyStreamer&) = delete;
+
+  int init() {
+    for (int b = 0; b < 2; b++) {
+      PB_CUDA(cudaMallocAsync((void**)&d_buf[b], kChunk, st));
+      h_buf[b] = (uint8_t*)pinned_scratch(kChunk, b);
+      if (!h_buf[b]) return fail(PB200_ERR_CUDA, "pinned staging buffer allocation failed");
+      PB_CUDA(cudaEventCreateWithFlags(&ev[b], cudaEventBlockingSync | cudaEventDisableTiming));
+    }
+    return 0;
+  }
+  // `count` Montgomery scalars at d_src -> count x 32 canonical bytes at dst
+  int scalars(const uint4* d_src, size_t count, uint8_t* dst) {
+    const size_t per = kChunk / 32;
+    for (size_t at = 0; at < count; at += per) PB_TRY(issue(d_src + 2 * at, std::min(per, count - at), dst + 32 * at, false));
+    return 0;
+  }
+  // `count` raw points at d_src -> count records of CommitKey::to_raw_var_bytes at dst
+  int points(const uint4* d_src, size_t count, uint8_t* dst) {
+    const size_t per = kChunk / 96;
+    for (size_t at = 0; at < count; at += per)
+      PB_TRY(issue(d_src + 6 * at, std::min(per, count - at), dst + (size_t)PB200_G1_RAW_SIZE * at, true));
+    return 0;
+  }
+  int finish() {
+    PB_TRY(drain(issued & 1));
+    return drain((issued & 1) ^ 1);
+  }
+
+ private:
+  // On entry at most the previous chunk is still pending, in the other pair of buffers.
+  int issue(const uint4* d_src, size_t count, uint8_t* dst, bool points) {
+    const int b = issued & 1;
+    if (points) {
+      PB_CUDA(cudaMemcpyAsync(h_buf[b], d_src, count * 96, cudaMemcpyDeviceToHost, st));
+    } else {
+      PB_LAUNCH(k_fr_to_canonical, div_up(count, 256), 256, 0, st, d_src, count, d_buf[b]);
+      PB_CUDA(cudaGetLastError());
+      PB_CUDA(cudaMemcpyAsync(h_buf[b], d_buf[b], count * 32, cudaMemcpyDeviceToHost, st));
+    }
+    PB_CUDA(cudaEventRecord(ev[b], st));
+    pend[b].dst = dst;
+    pend[b].count = count;
+    pend[b].points = points;
+    issued++;
+    return drain(b ^ 1);
+  }
+  int drain(int b) {
+    if (!pend[b].count) return 0;
+    const size_t count = pend[b].count;
+    pend[b].count = 0;
+    PB_CUDA(cudaEventSynchronize(ev[b]));
+    if (pend[b].points)
+      for (size_t i = 0; i < count; i++) raw_commit_key_record(h_buf[b] + 96 * i, pend[b].dst + (size_t)PB200_G1_RAW_SIZE * i);
+    else
+      memcpy(pend[b].dst, h_buf[b], count * 32);
+    return 0;
+  }
+};
+
+// Prover::to_bytes (src/compiler/prover.rs:212-263); the layout is spelled out at pb200_prover_from_bytes in
+// include/plonk_b200.h.  Reads only what the prover never changes after construction, on the caller's stream.
+int prover_to_bytes(const pb200_prover* P, uint8_t* out, size_t cap, size_t* len) {
+  cudaStream_t st = thread_stream();
+  const size_t n = P->n, n8 = P->n8, n_pts = srs_len(P->srs);
+  unsigned poly_len[N_POLY];
+  {
+    PoolBlock len_block(st);
+    PB_CUDA(len_block.alloc(sizeof poly_len));
+    PB_CUDA(cudaMemsetAsync(len_block.p, 0, sizeof poly_len, st));
+    PB_LAUNCH(k_poly_trim_len, dim3(div_up(n, 256), N_POLY), 256, 0, st, (const uint4*)P->d_polys, n, (unsigned*)len_block.p);
+    PB_CUDA(cudaGetLastError());
+    PB_CUDA(cudaMemcpyAsync(poly_len, len_block.p, sizeof poly_len, cudaMemcpyDeviceToHost, st));
+    PB_CUDA(stream_wait(st));
+  }
+  const size_t eval_size = n8 * 32 + 172, vk_len = 20 * 48 + 8, ck_len = 8 + n_pts * PB200_G1_RAW_SIZE;
+  size_t pk_len = 16 + 17 * eval_size;
+  for (int k = 0; k < N_POLY; k++) pk_len += 8 + 32 * (size_t)poly_len[k];
+  const size_t total = 48 + P->label.size() + pk_len + ck_len + vk_len;
+  *len = total;
+  if (!out) return 0;
+  if (cap < total) return fail(PB200_ERR_INVALID_ARG, "output buffer too small");
+
+  uint8_t* w = out;
+  auto be64 = [&](uint64_t v) {
+    for (int i = 7; i >= 0; i--) *w++ = (uint8_t)(v >> (8 * i));
+  };
+  auto le64 = [&](uint64_t v) {
+    for (int i = 0; i < 8; i++) *w++ = (uint8_t)(v >> (8 * i));
+  };
+  auto scalar = [&](const HFr& x) {  // BlsScalar::to_bytes
+    const HFr c = x.from_mont();
+    memcpy(w, c.v, 32);
+    w += 32;
+  };
+  // EvaluationDomain::to_bytes of the 8n domain (domain.rs:59-80), in front of every Evaluations
+  uint8_t domain[172];
+  {
+    w = domain;
+    le64(n8);
+    const uint32_t log8 = (uint32_t)P->log_n + 3;
+    for (int i = 0; i < 4; i++) *w++ = (uint8_t)(log8 >> (8 * i));
+    scalar(HFr::from_u64(n8));
+    scalar(to_host(ntt_size_inv(P->log_n + 3)));
+    scalar(to_host(ntt_group_gen(P->log_n + 3, false)));
+    scalar(to_host(ntt_group_gen(P->log_n + 3, true)));
+    scalar(to_host(ntt_coset_gen(true)));
+  }
+  KeyStreamer stream(st);
+  PB_TRY(stream.init());
+  auto evaluations = [&](const uint4* d_evals) {  // Evaluations::to_var_bytes (evaluations.rs:52-61)
+    memcpy(w, domain, sizeof domain);
+    w += sizeof domain;
+    uint8_t* at = w;
+    w += n8 * 32;
+    return stream.scalars(d_evals, n8, at);
+  };
+  w = out;
+  be64(P->label.size());
+  be64(pk_len);
+  be64(ck_len);
+  be64(vk_len);
+  be64(n);
+  be64(P->constraints);
+  memcpy(w, P->label.data(), P->label.size());
+  w += P->label.size();
+  // ProverKey::to_var_bytes (widget.rs:347-445)
+  le64(n);
+  le64(eval_size);
+  for (int i = 0; i < N_POLY; i++) {
+    const int k = kKeyFileOrder[i];
+    le64(poly_len[k]);
+    PB_TRY(stream.scalars(P->d_polys + 2 * (size_t)k * n, poly_len[k], w));
+    w += 32 * (size_t)poly_len[k];
+    PB_TRY(evaluations(P->d_key8 + 2 * (size_t)k * n8));
+  }
+  PB_TRY(evaluations(P->d_linear8));
+  {  // v_h_coset_8n (compiler.rs:424-425): (g w_8n^i)^n - 1 has period 8; the prover keeps only the inverses
+    memcpy(w, domain, sizeof domain);
+    w += sizeof domain;
+    uint8_t* base = w;
+    const HFr g = to_host(ntt_coset_gen(false)), w8n = to_host(ntt_group_gen(P->log_n + 3, false));
+    HFr point = g.pow_u64(n);
+    const HFr step = w8n.pow_u64(n);
+    for (int i = 0; i < 8; i++) {
+      scalar(point - HFr::one());
+      point = point * step;
+    }
+    for (size_t have = 256; have < n8 * 32; have *= 2) memcpy(base + have, base, have);  // n8 is 8 times a power of two
+    w = base + n8 * 32;
+  }
+  // CommitKey::to_raw_var_bytes (key.rs:215-229) of the trimmed key: window 0 of the MSM table holds the points as
+  // they were uploaded
+  le64(n_pts);
+  PB_TRY(stream.points(srs_points(P->srs), n_pts, w));
+  w += n_pts * PB200_G1_RAW_SIZE;
+  // VerifierKey::to_bytes (widget.rs:84-111)
+  le64(P->constraints);
+  for (int i = 0; i < N_POLY; i++) {
+    memcpy(w, P->comm[kKeyFileOrder[i]], 48);
+    w += 48;
+  }
+  memset(w, 0, vk_len - 8 - 48 * N_POLY);
+  return stream.finish();
 }
 
 void prover_free(pb200_prover* P) {
@@ -1280,6 +1502,12 @@ int pb200_prover_from_bytes(const uint8_t* bytes, size_t len, const uint32_t* wi
   PB_TRY(ensure_init());
   if (!bytes || !wires || !out) return fail(PB200_ERR_INVALID_ARG, "null argument");
   return prover_from_bytes(bytes, len, wires, n_witnesses, out);
+}
+
+int pb200_prover_to_bytes(const pb200_prover_t* p, uint8_t* out, size_t cap, size_t* len) {
+  if (!p || !len) return fail(PB200_ERR_INVALID_ARG, "null argument");
+  PB_TRY(ensure_init());
+  return prover_to_bytes(p, out, cap, len);
 }
 
 void pb200_prover_free(pb200_prover_t* p) {

@@ -53,13 +53,53 @@ def commit_key_bytes_of_public_parameters(raw_var_bytes: bytes) -> bytes:
     return raw_var_bytes[240:]
 
 
+_HOST_COMPRESS_MAX = 8  # up to this many points the per-point host encoder is quicker than a trip to the GPU
+
+
 def g1_compress(raw_points: bytes) -> bytes:
+    """N x 96-byte raw points -> N x 48-byte compressed points (G1Affine::to_bytes): one pb200_g1_compress_batch
+    call on the GPU, or the host encoder for a handful of points; the bytes are the same."""
+    n = len(raw_points) // G1_RAW_BYTES
+    if n > _HOST_COMPRESS_MAX:
+        out = ctypes.create_string_buffer(48 * n)
+        check(lib().pb200_g1_compress_batch(raw_points, n, out))
+        return out.raw
     out = ctypes.create_string_buffer(48)
     res = bytearray()
-    for i in range(0, len(raw_points), G1_RAW_BYTES):
+    for i in range(0, n * G1_RAW_BYTES, G1_RAW_BYTES):
         check(lib().pb200_g1_compress(raw_points[i : i + G1_RAW_BYTES], out))
         res += out.raw
     return bytes(res)
+
+
+def commit_key_to_var_bytes(raw_points: bytes) -> bytes:
+    """CommitKey::to_var_bytes (key.rs:303-308) of a key given as 96-byte raw points: the input of
+    CommitKey.from_slice."""
+    return g1_compress(raw_points)
+
+
+def commit_key_to_raw_var_bytes(raw_points: bytes) -> bytes:
+    """CommitKey::to_raw_var_bytes (key.rs:215-229): the input of CommitKey.from_raw_var_bytes and
+    from_slice_unchecked.  Host only."""
+    n = len(raw_points) // G1_RAW_BYTES
+    size = ctypes.c_size_t()
+    check(lib().pb200_commit_key_to_raw_var_bytes(raw_points or None, n, None, 0, ctypes.byref(size)))
+    out = ctypes.create_string_buffer(size.value)
+    check(lib().pb200_commit_key_to_raw_var_bytes(raw_points or None, n, out, size.value, ctypes.byref(size)))
+    return out.raw
+
+
+def public_parameters_to_var_bytes(opening_key: bytes, raw_points: bytes) -> bytes:
+    """PublicParameters::to_var_bytes (srs.rs:149-153): OpeningKey::to_bytes, then CommitKey::to_var_bytes."""
+    assert len(opening_key) == 240
+    return opening_key + commit_key_to_var_bytes(raw_points)
+
+
+def public_parameters_to_raw_var_bytes(opening_key: bytes, raw_points: bytes) -> bytes:
+    """PublicParameters::to_raw_var_bytes (srs.rs:114-119): OpeningKey::to_bytes, then
+    CommitKey::to_raw_var_bytes - what commit_key_bytes_of_public_parameters splits."""
+    assert len(opening_key) == 240
+    return opening_key + commit_key_to_raw_var_bytes(raw_points)
 
 
 class Commitment:
@@ -88,6 +128,15 @@ class CommitKey:
         h = ctypes.c_void_p()
         check(lib().pb200_srs_upload(raw_points, self.n_points, ctypes.byref(h)))
         self._h = h
+        self._raw = bytes(raw_points)  # the writers below re-encode the points the key was made from
+
+    def to_var_bytes(self) -> bytes:
+        """CommitKey::to_var_bytes (key.rs:303-308): 48 compressed bytes per point, encoded on the GPU."""
+        return commit_key_to_var_bytes(self._raw)
+
+    def to_raw_var_bytes(self) -> bytes:
+        """CommitKey::to_raw_var_bytes (key.rs:215-229)."""
+        return commit_key_to_raw_var_bytes(self._raw)
 
     @classmethod
     def from_slice(cls, compressed: bytes) -> "CommitKey":

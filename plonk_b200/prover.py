@@ -43,6 +43,20 @@ class Prover:
         self.n_witnesses = n_witnesses
         return self
 
+    def serialized_size(self) -> int:
+        """Prover::serialized_size (prover.rs:233-235)."""
+        n = ctypes.c_size_t()
+        check(lib().pb200_prover_to_bytes(self._h, None, 0, ctypes.byref(n)))
+        return n.value
+
+    def to_bytes(self) -> bytes:
+        """Prover::to_bytes (prover.rs:238-263): what from_bytes reads, here or in another process; the scalars are
+        converted to canonical form on the GPU.  Safe beside proofs running on this prover."""
+        n = ctypes.c_size_t(self.serialized_size())
+        out = ctypes.create_string_buffer(n.value)
+        check(lib().pb200_prover_to_bytes(self._h, out, n.value, ctypes.byref(n)))
+        return out.raw
+
     def commitments(self):
         out = ctypes.create_string_buffer(15 * 48)
         check(lib().pb200_prover_commitments(self._h, out))
