@@ -6,10 +6,8 @@
 #include <mutex>
 #include <vector>
 
-#include "common.cuh"
+#include "internal.cuh"
 #include "host_field.h"
-
-struct pb200_srs;
 
 namespace pb {
 thread_local std::string g_last_error;
@@ -95,35 +93,6 @@ void* pinned_scratch(size_t bytes, int slot) {
   return buf;
 }
 
-int ntt_run(const uint64_t* d_in, size_t in_len, uint64_t* d_out, uint32_t log_n, int inverse, int coset,
-            uint32_t batch, size_t in_stride, size_t out_stride, cudaStream_t st, Arena* ar);
-int msm_run(const pb200_srs* srs, size_t first, const uint64_t* d_scalars, size_t n, uint32_t batch,
-            size_t stride, uint64_t* out_affine_host, cudaStream_t st, Arena* ar);
-int srs_upload(const uint8_t* raw, size_t n_points, pb200_srs** out, int window_bits);
-typedef int (*nccl_all_gather_fn)(const void*, void*, size_t, int, void*, cudaStream_t);
-int msm_allgather(const pb200_srs* srs, const uint64_t* scalars, bool scalars_on_device, size_t n, uint32_t batch, size_t stride,
-                  nccl_all_gather_fn all_gather, void* comm, int n_ranks, int* nccl_rc, uint64_t* out_affine_host, cudaStream_t st);
-int msm_combine_parts(const uint32_t* parts, int n_parts, int window_bits, uint32_t batch, uint64_t* out_affine_host, size_t* words_per_entry);
-int selftest_mul(int which, const uint64_t* a, const uint64_t* b, uint64_t* o, size_t n);
-int imad_peak(double* out);
-int fp_product_peak(double* out);
-int lagrange_key_dev(const uint4* d_in, int log_n, uint4* d_out, cudaStream_t st);
-int selftest_fp_ops(const uint64_t* a, const uint64_t* b, const uint64_t* c, const uint64_t* d, uint64_t* o, size_t n);
-size_t srs_len(const pb200_srs* s);
-int srs_window(const pb200_srs* s);
-int msm_window_for(size_t n_points);
-int srs_setup(const uint64_t* x_mont, const uint64_t* g_scalar_mont, size_t n, uint8_t* out_raw);
-int g1_decompress(const uint8_t* in, size_t n, int check_subgroup, uint8_t* out_raw);
-int g1_check_raw(const uint8_t* raw, size_t n);
-int g1_compress_batch(const uint8_t* raw, size_t n, uint8_t* out_48);
-int raw_commit_key_parse(const uint8_t* bytes, size_t len, int checked, size_t* n_points, uint8_t* out_raw);
-extern std::atomic<int> g_prof_on;
-extern std::atomic<uint64_t> g_prof_acc_ns, g_prof_acc_adds, g_prof_acc_launches, g_prof_acc_points;
-extern std::atomic<uint64_t> g_prof_sp_ns, g_prof_sp_adds, g_prof_sp_launches, g_prof_sp_points;
-void srs_free(pb200_srs* s);
-}  // namespace pb
-
-namespace pb {
 // checked = 1: CommitKey::from_raw_var_bytes (key.rs:258-298: the length must be exact, zero points are an
 // error); checked = 0: from_slice_unchecked (key.rs:242-256: as many whole records as the bytes hold, at most
 // the announced count).  Writes the 96-byte layout when out_raw is given (identity -> zeros).
@@ -255,7 +224,7 @@ int pb200_msm_g1_dev(const pb200_srs_t* srs, const uint64_t* d_scalars, size_t n
   PB_TRY(ensure_init());
   if (!srs || !out_affine_host) return fail(PB200_ERR_INVALID_ARG, "null argument");
   cudaStream_t st = stream ? (cudaStream_t)stream : thread_stream();
-  return msm_run(srs, 0, d_scalars, n_scalars, batch, stride, out_affine_host, st, nullptr);
+  return msm_run(srs, 0, d_scalars, n_scalars, batch, stride, kMsmLatency, out_affine_host, st, nullptr);
 }
 
 static int msm_host(const pb200_srs_t* srs, size_t first, const uint64_t* scalars, size_t n, uint32_t batch,
@@ -270,7 +239,7 @@ static int msm_host(const pb200_srs_t* srs, size_t first, const uint64_t* scalar
     PB_ALLOC(scope, d, (size_t)batch * n * 32);
     PB_CUDA(cudaMemcpy2DAsync(d, n * 32, scalars, stride * 32, n * 32, batch, cudaMemcpyHostToDevice, st));
   }
-  return msm_run(srs, first, d, n, batch, n, out, st, nullptr);
+  return msm_run(srs, first, d, n, batch, n, kMsmLatency, out, st, nullptr);
 }
 
 int pb200_msm_g1(const pb200_srs_t* srs, const uint64_t* scalars, size_t n_scalars, uint32_t batch, size_t stride,
@@ -287,10 +256,9 @@ int pb200_msm_g1_range(const pb200_srs_t* srs, size_t first, const uint64_t* sca
 // communicator was created with when one is already loaded), so that the library itself carries no
 // NCCL dependency and loads on hosts without it.
 namespace {
-typedef int (*nccl_all_gather_t)(const void*, void*, size_t, int, void*, cudaStream_t);
 typedef const char* (*nccl_error_string_t)(int);
 struct NcclApi {
-  nccl_all_gather_t all_gather = nullptr;
+  nccl_all_gather_fn all_gather = nullptr;
   nccl_error_string_t error_string = nullptr;
 };
 const NcclApi* nccl_api() {
@@ -298,7 +266,7 @@ const NcclApi* nccl_api() {
     NcclApi a;
     void* h = dlopen("libnccl.so.2", RTLD_NOW | RTLD_GLOBAL);
     if (h) {
-      a.all_gather = (nccl_all_gather_t)dlsym(h, "ncclAllGather");
+      a.all_gather = (nccl_all_gather_fn)dlsym(h, "ncclAllGather");
       a.error_string = (nccl_error_string_t)dlsym(h, "ncclGetErrorString");
     }
     return a;

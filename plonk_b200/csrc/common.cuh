@@ -70,8 +70,10 @@ inline unsigned num_sms() { return g_num_sms.load(std::memory_order_relaxed); }
 struct Arena {
   char* base = nullptr;
   size_t size = 0, off = 0;
+  // Blocks start 256-byte aligned, so a list of blocks fits in the sum of round_up(bytes) over the list.
+  static size_t round_up(size_t bytes) { return (bytes + 255) & ~(size_t)255; }
   void* take(size_t bytes) {
-    const size_t a = (off + 255) & ~(size_t)255;
+    const size_t a = round_up(off);
     if (a + bytes > size) return nullptr;
     off = a + bytes;
     return base + a;

@@ -1,18 +1,14 @@
 // Lagrange form of a commit key on the GPU: inverse NTT over G1 points (csrc/ecntt.cuh).
 //
-// Not used by the prover yet (DESIGN.md, next steps: wire commitments in the Lagrange basis); exposed
-// as pb200_g1_lagrange_key so that the transform can be checked on its own.  One thread per butterfly,
-// log n launches; a butterfly is one XYZZ addition, one subtraction and a 255-bit double-and-add
-// (~380 group operations), so the whole transform is ~n/2 log n * 380 group operations - about 2e8
-// at n = 2^16 - once per key.
-#include "common.cuh"
+// prover_build (prover.cu) makes the Lagrange-form key of the wire commitments with it; it is also
+// exposed as pb200_g1_lagrange_key so that the transform can be checked on its own.  One thread per
+// butterfly, log n launches; a butterfly is one XYZZ addition, one subtraction and a 255-bit
+// double-and-add (~380 group operations), so the whole transform is ~n/2 log n * 380 group
+// operations - about 2e8 at n = 2^16 - once per key.
+#include "internal.cuh"
 #include "ecntt.cuh"
 
 namespace pb {
-
-int get_twiddles(int logm, bool inverse, cudaStream_t st, const uint4** out);
-Fr ntt_size_inv(int log_n);
-
 namespace {
 
 PB_D Fp ec_ld_fp(const uint4* q) {

@@ -25,7 +25,7 @@
 #include <atomic>
 #include <vector>
 
-#include "common.cuh"
+#include "internal.cuh"
 #include "fp_inv.cuh"
 #include "g1.cuh"
 #include "host_field.h"
@@ -1128,13 +1128,6 @@ static void xyzz_dev_to_host(const uint32_t* w, pbh::HXyzz* o) {
   memcpy(o->zzz.v, w + 36, 48);
 }
 
-// Set by a caller that keeps several MSMs in flight on other streams (prover.cu): dense MSMs then use one lane
-// per bucket (no merge additions).  Thread-local: an MSM is enqueued by the thread that owns its stream.
-thread_local int t_msm_throughput_hint = 0;
-// Set by the same caller for an MSM that keeps its latency-oriented bucket split (the sparse wire MSM) while other
-// proofs are in flight: only its over-long buckets switch to the wide chunks.
-thread_local int t_msm_wide_heavy_chunks = 0;
-
 // What the host needs to finish an MSM whose kernels have been enqueued: the digit plan of the bucket
 // reduction.  It depends on the window width of the key only, never on the number of scalars, so the
 // ranks of a point-sharded MSM (pb200_msm_g1_allgather*) share it as long as their slices use the same c.
@@ -1166,7 +1159,7 @@ static size_t aff_slots(size_t cap, size_t nb) {
   return widest * (kAffK / 2);
 }
 
-static int msm_plan_c(int c, uint32_t batch, MsmTail* tail, unsigned* n_groups_out, int* g_out) {
+static int msm_plan(int c, uint32_t batch, MsmTail* tail) {
   const unsigned nb = 1u << (c - 1);
   const int g = std::min<unsigned>(kGroup, nb);
   const unsigned n_groups = nb / g;
@@ -1192,12 +1185,7 @@ static int msm_plan_c(int c, uint32_t batch, MsmTail* tail, unsigned* n_groups_o
   tail->log_g = log_g;
   tail->c = c;
   tail->batch = batch;
-  *n_groups_out = n_groups;
-  *g_out = g;
   return 0;
-}
-static int msm_plan(const pb200_srs* srs, uint32_t batch, MsmTail* tail, unsigned* n_groups_out, int* g_out) {
-  return msm_plan_c(srs->c, batch, tail, n_groups_out, g_out);
 }
 
 // kListChunk-member chunks of the longest list of k_msm_lists (n_parts partials per column)
@@ -1207,96 +1195,126 @@ static unsigned reduction_chunks(const DigitPlan& plan, unsigned n_groups, unsig
   return std::max(chunks, 1u);
 }
 
+// The scratch buffers of msm_enqueue in carving order; the kAff* ones exist under PB200_MSM_AFFINE=1 only.
+enum MsmBuf { kResult, kCounts, kOffsets, kOrder, kMaxLen, kNHeavy, kHeavyPre, kEbkt, kEpos, kSorted, kSums, kLists, kS, kP,
+              kPartials, kAffA, kAffB, kAffPre, kAffDesc, kAffFactor, kAffNpairs, kAffCtot, kAffCpre, kMsmBufs };
+
+// What `batch` MSMs of n scalars against a key of window c (W windows) are sized from: the reduction plan, the extents
+// the kernels take and the bytes of every buffer.  msm_enqueue carves exactly `bytes`; msm_workspace_bytes adds them up.
+struct MsmScratch {
+  MsmTail tail;
+  unsigned n_groups = 0, col_run = 0, n_parts = 0, chunks = 0, ctas_max = 0;
+  int g = 0;
+  size_t part_cap = 0, cap_a = 0, cap_b = 0, slots = 0;
+  size_t bytes[kMsmBufs] = {};
+};
+static int msm_scratch(int c, int W, size_t n, uint32_t batch, bool affine, MsmScratch* s) {
+  PB_TRY(msm_plan(c, batch, &s->tail));
+  const DigitPlan& plan = s->tail.plan;
+  const size_t nb = (size_t)1 << (c - 1), cap = n * (size_t)W, B = batch;
+  s->g = 1 << s->tail.log_g;  // buckets per row of the reduction
+  s->n_groups = (unsigned)(nb >> s->tail.log_g);
+  s->col_run = std::min(kColRun, s->n_groups);
+  s->n_parts = s->n_groups / s->col_run;
+  s->chunks = reduction_chunks(plan, s->n_groups, s->n_parts);
+  // chunk sums of the heavy buckets: at most cap / kHeavyChunk full chunks (the narrower chunk bounds both shapes)
+  // plus one ragged chunk per heavy bucket
+  s->part_cap = cap / kHeavyChunk + std::min<size_t>(nb, cap / kHeavyMin) + 2;
+  size_t* b = s->bytes;
+  b[kResult] = B * (plan.ndig + 1) * 192;
+  b[kCounts] = b[kOrder] = B * nb * 4;
+  b[kOffsets] = b[kHeavyPre] = B * (nb + 1) * 4;
+  b[kMaxLen] = b[kNHeavy] = B * 4;
+  b[kEbkt] = b[kEpos] = b[kSorted] = B * cap * 4;
+  b[kSums] = B * nb * 192;
+  b[kLists] = B * plan.nlists * s->chunks * 192;
+  b[kS] = B * s->n_groups * 192;
+  b[kP] = B * s->g * s->n_parts * 192;
+  b[kPartials] = B * s->part_cap * 192;
+  if (affine) {  // two point buffers for the pairwise rounds, running products and pair descriptors, CTA totals
+    s->cap_a = cap / 2 + nb + 2;
+    s->cap_b = cap / 4 + nb + 2;
+    s->slots = aff_slots(cap, nb);
+    const size_t threads_max = s->slots / (kAffK / 2);
+    s->ctas_max = (unsigned)(threads_max / kAffThreads);
+    b[kAffA] = B * s->cap_a * 96;
+    b[kAffB] = B * s->cap_b * 96;
+    b[kAffPre] = B * s->slots * 48;
+    b[kAffDesc] = B * s->slots * 16;
+    b[kAffFactor] = B * threads_max * 48;
+    b[kAffNpairs] = B * threads_max * 4;
+    b[kAffCtot] = b[kAffCpre] = B * s->ctas_max * 48;
+  }
+  return 0;
+}
+
 // Enqueues every kernel of `batch` MSMs over the points [first, first + n) of the key on `st`.  The
 // digit sums land in *d_result ([batch][ndig + 1] XYZZ points, carved from `scope`, so they live until
 // the scope is released); nothing is synchronised.  n == 0 yields identities.
 static int msm_enqueue(const pb200_srs* srs, size_t first, const uint64_t* d_scalars, size_t n, uint32_t batch, size_t stride,
-                       cudaStream_t st, ScratchScope& scope, uint4** d_result, MsmTail* tail, cudaEvent_t* prof_ev,
+                       MsmShape shape, cudaStream_t st, ScratchScope& scope, uint4** d_result, MsmTail* tail, cudaEvent_t* prof_ev,
                        const unsigned** d_totals) {
   if (first + n > srs->n_points) return fail(PB200_ERR_DEGREE_TOO_LARGE, "more scalars than commit-key points");
   const int c = srs->c, W = srs->W;
   const unsigned nb = 1u << (c - 1);
   const size_t cap = n * (size_t)W;
   if (((srs->n_points * (size_t)W) << 1) >= ((size_t)1 << 32)) return fail(PB200_ERR_INVALID_ARG, "commit key too large for 32-bit point references");
-  unsigned n_groups = 0;
-  int g = 0;
-  PB_TRY(msm_plan(srs, batch, tail, &n_groups, &g));
+  const bool affine = msm_affine_enabled();
+  MsmScratch s;
+  PB_TRY(msm_scratch(c, W, n, batch, affine, &s));
+  *tail = s.tail;
   const DigitPlan& plan = tail->plan;
+  const unsigned n_groups = s.n_groups, col_run = s.col_run, n_parts = s.n_parts, chunks = s.chunks;
+  const int g = s.g;
   uint4* result = nullptr;
-  PB_ALLOC(scope, result, (size_t)batch * (plan.ndig + 1) * 192);
+  PB_ALLOC(scope, result, s.bytes[kResult]);
   *d_result = result;
   if (n == 0) {
-    PB_CUDA(cudaMemsetAsync(result, 0, (size_t)batch * (plan.ndig + 1) * 192, st));
+    PB_CUDA(cudaMemsetAsync(result, 0, s.bytes[kResult], st));
     return 0;
   }
 
   // threads per bucket: enough CTAs to fill the machine, but at least ~8 points per thread.  Splitting a bucket
   // over 2^k lanes costs k full additions per bucket for the merge (+39 % work at k = 2 with 32 entries per
   // bucket): it buys latency when the launch is alone on the GPU and only costs throughput when other proofs
-  // keep the machine busy - the caller says which (t_msm_throughput_hint, set by the prover from its number of
-  // proofs in flight).
+  // keep the machine busy - the caller says which (shape.split_buckets).
   int log_split = 0;
-  if (!t_msm_throughput_hint) {
+  if (shape.split_buckets) {
     const size_t avg = cap / nb;
     while (log_split < 5 && ((size_t)nb * batch << log_split) < (1u << 17) && (avg >> (log_split + 1)) >= 8) log_split++;
   }
   if (const char* env = getenv("PB200_MSM_LOG_SPLIT")) log_split = atoi(env);
 
-  unsigned *counts = nullptr, *offsets = nullptr, *order = nullptr, *ebkt = nullptr, *epos = nullptr, *sorted = nullptr;
-  uint4 *sums = nullptr, *lists = nullptr, *S = nullptr, *P = nullptr;
-  PB_ALLOC(scope, counts, (size_t)batch * nb * 4);
-  PB_ALLOC(scope, offsets, (size_t)batch * (nb + 1) * 4);
-  PB_ALLOC(scope, order, (size_t)batch * nb * 4);
-  const bool affine = msm_affine_enabled();
-  unsigned *n_heavy = nullptr, *heavy_pre = nullptr, *max_len = nullptr;
-  PB_ALLOC(scope, max_len, (size_t)batch * 4);
-  PB_ALLOC(scope, n_heavy, (size_t)batch * 4);
-  PB_ALLOC(scope, heavy_pre, (size_t)batch * (nb + 1) * 4);
-  PB_ALLOC(scope, ebkt, (size_t)batch * cap * 4);
-  PB_ALLOC(scope, epos, (size_t)batch * cap * 4);
-  PB_ALLOC(scope, sorted, (size_t)batch * cap * 4);
-  PB_ALLOC(scope, sums, (size_t)batch * nb * 192);
-  const unsigned col_run = std::min(kColRun, n_groups), n_parts = n_groups / col_run;
-  const unsigned chunks = reduction_chunks(plan, n_groups, n_parts);
-  PB_ALLOC(scope, lists, (size_t)batch * plan.nlists * chunks * 192);
-  PB_ALLOC(scope, S, (size_t)batch * n_groups * 192);
-  PB_ALLOC(scope, P, (size_t)batch * g * n_parts * 192);
-  PB_CUDA(cudaMemsetAsync(counts, 0, (size_t)batch * nb * 4, st));
+  void* buf[kMsmBufs] = {};
+  for (int i = kCounts; i < (affine ? kMsmBufs : kAffA); i++) PB_ALLOC(scope, buf[i], s.bytes[i]);
+  unsigned *counts = (unsigned*)buf[kCounts], *offsets = (unsigned*)buf[kOffsets], *order = (unsigned*)buf[kOrder],
+           *max_len = (unsigned*)buf[kMaxLen], *n_heavy = (unsigned*)buf[kNHeavy], *heavy_pre = (unsigned*)buf[kHeavyPre],
+           *ebkt = (unsigned*)buf[kEbkt], *epos = (unsigned*)buf[kEpos], *sorted = (unsigned*)buf[kSorted];
+  uint4 *sums = (uint4*)buf[kSums], *lists = (uint4*)buf[kLists], *S = (uint4*)buf[kS], *P = (uint4*)buf[kP],
+        *partials = (uint4*)buf[kPartials];
+  PB_CUDA(cudaMemsetAsync(counts, 0, s.bytes[kCounts], st));
 
   PB_LAUNCH(k_msm_digits, dim3(div_up(n, 128), batch), 128, 0, st, (const uint4*)d_scalars, n, stride, c, W, nb,
             counts, ebkt, epos);
   int size_shift = 0;  // size unit: average bucket ~ 64 units
   while (((cap / nb) >> size_shift) > 64) size_shift++;
-  // chunk sums of the heavy buckets: at most cap / heavy_chunk full chunks plus one ragged chunk per heavy bucket
-  const unsigned heavy_chunk = (t_msm_throughput_hint || t_msm_wide_heavy_chunks) ? kHeavyChunkWide : kHeavyChunk;
-  const size_t part_cap = cap / kHeavyChunk + std::min<size_t>(nb, cap / kHeavyMin) + 2;
-  uint4* partials = nullptr;
-  PB_ALLOC(scope, partials, (size_t)batch * part_cap * 192);
+  const unsigned heavy_chunk = shape.wide_heavy_chunks ? kHeavyChunkWide : kHeavyChunk;
+  const size_t part_cap = s.part_cap;
   PB_LAUNCH(k_msm_scan, batch, 1024, 0, st, counts, offsets, order, n_heavy, heavy_pre, max_len, nb, size_shift, heavy_chunk);
   PB_LAUNCH(k_msm_scatter, dim3(div_up(n, 256), W, batch), 256, 0, st, ebkt, epos, offsets, n, W, nb,
             srs->n_points, first, sorted);
   if (prof_ev) PB_CUDA(cudaEventRecord(prof_ev[0], st));
   if (affine) {
     // batched-affine pairwise rounds (see k_msm_affine_fwd)
-    const size_t capA = cap / 2 + nb + 2, capB = cap / 4 + nb + 2;
+    const size_t capA = s.cap_a, capB = s.cap_b, slots = s.slots;
+    const unsigned ctas_max = s.ctas_max;
     int rounds = 0;
     while (((size_t)1 << rounds) < cap) rounds++;  // a bucket can hold every entry (equal scalars with equal digits)
     // input positions of round r: layout 0 is exact, layout r >= 1 has at most one slot of slack per bucket
     auto positions = [&](int r) { return r == 0 ? cap : (cap >> r) + nb + 1; };
-    const size_t slots = aff_slots(cap, nb);
-    uint4 *bufA = nullptr, *bufB = nullptr, *pre = nullptr, *factor = nullptr, *ctot = nullptr, *cpre = nullptr;
-    uint4* desc = nullptr;
-    unsigned* npairs = nullptr;
-    const size_t threads_max = slots / (kAffK / 2);
-    const unsigned ctas_max = (unsigned)(threads_max / kAffThreads);
-    PB_ALLOC(scope, bufA, (size_t)batch * capA * 96);
-    PB_ALLOC(scope, bufB, (size_t)batch * capB * 96);
-    PB_ALLOC(scope, pre, (size_t)batch * slots * 48);
-    PB_ALLOC(scope, desc, (size_t)batch * slots * 16);
-    PB_ALLOC(scope, factor, (size_t)batch * threads_max * 48);
-    PB_ALLOC(scope, npairs, (size_t)batch * threads_max * 4);
-    PB_ALLOC(scope, ctot, (size_t)batch * ctas_max * 48);
-    PB_ALLOC(scope, cpre, (size_t)batch * ctas_max * 48);
+    uint4 *bufA = (uint4*)buf[kAffA], *bufB = (uint4*)buf[kAffB], *pre = (uint4*)buf[kAffPre], *desc = (uint4*)buf[kAffDesc],
+          *factor = (uint4*)buf[kAffFactor], *ctot = (uint4*)buf[kAffCtot], *cpre = (uint4*)buf[kAffCpre];
+    unsigned* npairs = (unsigned*)buf[kAffNpairs];
     PB_CUDA(cudaMemsetAsync(sums, 0, (size_t)batch * nb * 96, st));
     for (int r = 0; r < rounds; r++) {
       AffRound a;
@@ -1415,16 +1433,14 @@ static void msm_finish(const uint32_t* host, const MsmTail& tail, int n_parts, u
 // The host tail on its own (pb200_msm_combine_parts): digit sums of n_parts partial MSMs -> affine results.
 int msm_combine_parts(const uint32_t* parts, int n_parts, int window_bits, uint32_t batch, uint64_t* out_affine_host, size_t* words_per_entry) {
   MsmTail tail;
-  unsigned n_groups = 0;
-  int g = 0;
-  PB_TRY(msm_plan_c(window_bits, batch, &tail, &n_groups, &g));
+  PB_TRY(msm_plan(window_bits, batch, &tail));
   if (words_per_entry) *words_per_entry = tail.words_per_entry();
   if (parts && out_affine_host) msm_finish(parts, tail, n_parts, out_affine_host);
   return 0;
 }
 
-int msm_run(const pb200_srs* srs, size_t first, const uint64_t* d_scalars, size_t n, uint32_t batch,
-            size_t stride, uint64_t* out_affine_host, cudaStream_t st, Arena* ar) {
+int msm_run(const pb200_srs* srs, size_t first, const uint64_t* d_scalars, size_t n, uint32_t batch, size_t stride,
+            MsmShape shape, uint64_t* out_affine_host, cudaStream_t st, Arena* ar) {
   if (first + n > srs->n_points) return fail(PB200_ERR_DEGREE_TOO_LARGE, "more scalars than commit-key points");
   if (batch == 0) return 0;
   if (n == 0) {
@@ -1448,7 +1464,7 @@ int msm_run(const pb200_srs* srs, size_t first, const uint64_t* d_scalars, size_
   uint4* result = nullptr;
   MsmTail tail;
   const unsigned* d_totals = nullptr;
-  PB_TRY(msm_enqueue(srs, first, d_scalars, n, batch, stride, st, scope, &result, &tail, prof ? ev : nullptr, &d_totals));
+  PB_TRY(msm_enqueue(srs, first, d_scalars, n, batch, stride, shape, st, scope, &result, &tail, prof ? ev : nullptr, &d_totals));
   std::vector<unsigned> h_tot(batch, 0);
   if (prof) {
     const unsigned nb = 1u << (srs->c - 1);
@@ -1481,13 +1497,10 @@ int msm_run(const pb200_srs* srs, size_t first, const uint64_t* d_scalars, size_
 // straight behind the reduction kernels: there is one host synchronisation per call.  Every rank's
 // record starts with a 16-byte header {status, c, ndig, batch}; a rank whose local part failed still
 // joins the collective with status != 0, so its peers return an error instead of hanging.
-typedef int (*nccl_all_gather_fn)(const void*, void*, size_t, int, void*, cudaStream_t);
 int msm_allgather(const pb200_srs* srs, const uint64_t* scalars, bool scalars_on_device, size_t n, uint32_t batch, size_t stride,
                   nccl_all_gather_fn all_gather, void* comm, int n_ranks, int* nccl_rc, uint64_t* out_affine_host, cudaStream_t st) {
   MsmTail tail;
-  unsigned n_groups = 0;
-  int g = 0;
-  PB_TRY(msm_plan(srs, batch, &tail, &n_groups, &g));
+  PB_TRY(msm_plan(srs->c, batch, &tail));
   const size_t payload = (size_t)batch * tail.words_per_entry() * 4, rec = 16 + payload;
   ScratchScope scope(nullptr, st);
   uint8_t *d_send = nullptr, *d_recv = nullptr;
@@ -1509,7 +1522,7 @@ int msm_allgather(const pb200_srs* srs, const uint64_t* scalars, bool scalars_on
       d_scalars = d;
       stride = n;
     }
-    if (local_rc == 0) local_rc = msm_enqueue(srs, 0, d_scalars, n, batch, stride, st, scope, &result, &t2, nullptr, nullptr);
+    if (local_rc == 0) local_rc = msm_enqueue(srs, 0, d_scalars, n, batch, stride, kMsmLatency, st, scope, &result, &t2, nullptr, nullptr);
     cudaError_t e = cudaSuccess;
     if (local_rc == 0) e = cudaMemcpyAsync(d_send + 16, result, payload, cudaMemcpyDeviceToDevice, st);
     if (local_rc != 0 || e != cudaSuccess) {
@@ -1550,34 +1563,13 @@ int msm_allgather(const pb200_srs* srs, const uint64_t* scalars, bool scalars_on
   return 0;
 }
 
-// Upper bound of the arena bytes one msm_run(n, batch) call takes (same list as the PB_ALLOCs above).
+// The arena bytes one msm_run(n, batch) call carves, in either shape.
 size_t msm_workspace_bytes(const pb200_srs* srs, size_t n, uint32_t batch) {
-  const size_t nb = (size_t)1 << (srs->c - 1), cap = n * (size_t)srs->W;
-  MsmTail tail;
-  unsigned n_groups = 0;
-  int g = 0;
-  if (msm_plan(srs, batch, &tail, &n_groups, &g) != 0) return 0;
-  const unsigned n_parts = n_groups / std::min(kColRun, n_groups);
-  size_t b = 0;
-  b += 4 * ((size_t)batch * (nb + 1) * 4 + 256);      // counts, offsets, order, heavy_pre
-  {
-    int size_shift = 0;
-    while (((cap / nb) >> size_shift) > 64) size_shift++;
-    b += (size_t)batch * (cap / kHeavyChunk + std::min<size_t>(nb, cap / kHeavyMin) + 2) * 192 + 256;  // partials
-  }
-  b += (size_t)batch * 4 + 256;                        // n_heavy
-  b += 3 * ((size_t)batch * cap * 4 + 256);            // ebkt, epos, sorted
-  b += (size_t)batch * nb * 192 + 256;                 // sums
-  b += (size_t)batch * n_groups * 192 + 256;           // S
-  b += (size_t)batch * g * n_parts * 192 + 256;        // P
-  b += (size_t)batch * tail.plan.nlists * reduction_chunks(tail.plan, n_groups, n_parts) * 192 + 256;  // lists x chunks
-  b += (size_t)batch * 9 * 192 + 256;                  // result
-  if (msm_affine_enabled()) {  // batched-affine rounds: two point buffers, running products, pair descriptors
-    b += (size_t)batch * ((cap / 2 + nb + 2) + (cap / 4 + nb + 2)) * 96 + 512;
-    b += (size_t)batch * aff_slots(cap, nb) * (48 + 16) + 512;
-    b += (size_t)batch * (aff_slots(cap, nb) / (kAffK / 2)) * (48 + 4 + 1) + 2048;  // factor, npairs, CTA totals
-  }
-  return b + 4096;
+  MsmScratch s;
+  if (msm_scratch(srs->c, srs->W, n, batch, msm_affine_enabled(), &s) != 0) return 0;
+  size_t total = 0;
+  for (size_t b : s.bytes) total += Arena::round_up(b);
+  return total;
 }
 
 int srs_upload(const uint8_t* raw, size_t n_points, pb200_srs** out, int window_bits) {
@@ -1606,8 +1598,6 @@ int srs_upload(const uint8_t* raw, size_t n_points, pb200_srs** out, int window_
   *out = s;
   return 0;
 }
-
-int srs_upload(const uint8_t* raw, size_t n_points, pb200_srs** out) { return srs_upload(raw, n_points, out, 0); }
 
 // The key's points as uploaded (window 0 of the table), n_points affine points on the device.
 const uint4* srs_points(const pb200_srs* s) { return s->table; }

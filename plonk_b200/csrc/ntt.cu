@@ -23,7 +23,7 @@
 #include <mutex>
 #include <vector>
 
-#include "common.cuh"
+#include "internal.cuh"
 
 namespace pb {
 

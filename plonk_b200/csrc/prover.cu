@@ -21,40 +21,16 @@
 #include <mutex>
 #include <vector>
 
-#include "common.cuh"
+#include "internal.cuh"
 #include "host_field.h"
 #include "plonk_algebra.cuh"
 #include "transcript.h"
 
-struct pb200_srs;
-
 namespace pb {
 
-int ntt_run(const uint64_t* d_in, size_t in_len, uint64_t* d_out, uint32_t log_n, int inverse, int coset,
-            uint32_t batch, size_t in_stride, size_t out_stride, cudaStream_t st, Arena* ar);
-int msm_run(const pb200_srs* srs, size_t first, const uint64_t* d_scalars, size_t n, uint32_t batch,
-            size_t stride, uint64_t* out_affine_host, cudaStream_t st, Arena* ar);
-size_t msm_workspace_bytes(const pb200_srs* srs, size_t n, uint32_t batch);
-int srs_upload(const uint8_t* raw, size_t n_points, pb200_srs** out);
-void srs_free(pb200_srs* s);
-size_t srs_len(const pb200_srs* s);
-const uint4* srs_points(const pb200_srs* s);
-int srs_from_device(const uint4* d_points, size_t n_points, pb200_srs** out, int window_bits);
-int msm_window_for(size_t n_points);
-extern thread_local int t_msm_throughput_hint;
-extern thread_local int t_msm_wide_heavy_chunks;
 // pb200_throughput_mode(1): treat every proof as one of many in flight (a measurement aid: bench.py times the
 // dominant kernel with single proofs but wants the launch shape of its timed region)
 static std::atomic<int> g_force_throughput{0};
-int g1_check_raw(const uint8_t* raw, size_t n);
-int raw_commit_key_parse(const uint8_t* bytes, size_t len, int checked, size_t* n_points, uint8_t* out_raw);
-void raw_commit_key_record(const uint8_t* raw96, uint8_t* rec97);
-int lagrange_key_dev(const uint4* d_in, int log_n, uint4* d_out, cudaStream_t st);
-int get_twiddles(int logm, bool inverse, cudaStream_t st, const uint4** out);
-int fill_powers(uint4* out, size_t n, const Fr& base, const Fr& scale, cudaStream_t st);
-Fr ntt_group_gen(int log_n, bool inverse);
-Fr ntt_size_inv(int log_n);
-Fr ntt_coset_gen(bool inverse);
 
 PB_D Fr ldg_fr(const uint4* p, size_t i) {
   uint4 a = __ldg(p + 2 * i), b = __ldg(p + 2 * i + 1);
@@ -622,6 +598,26 @@ static int fr_scan(const uint4* in, size_t n, uint4* out, cudaStream_t st, Arena
   PB_CUDA(cudaGetLastError());
   return 0;
 }
+static size_t fr_scan_bytes(size_t n) {  // the arena bytes fr_scan(n) carves, by the same recursion
+  const size_t nblk = div_up(n, 2048);
+  return 2 * Arena::round_up(nblk * 32) + (nblk > 1 ? fr_scan_bytes(nblk) : 0);
+}
+
+// The buffers prove_dev keeps for a whole proof, in carving order; prover_build sizes the arena from the same list.
+enum ProofBuf { kWv, kZp, kNum, kDen, kW8, kQuot, kTcoef, kTq, kAgg, kPw, kScratch, kEvals, kPartial, kFlag, kProofBufs };
+static void proof_buffers(size_t n, size_t bytes[kProofBufs]) {
+  const size_t stride = n + 8;
+  bytes[kWv] = 5 * n * 32;       // wire values a, b, c, d and the dense public-input vector
+  bytes[kZp] = 6 * stride * 32;  // [z, a, b, c, d, pi] coefficient form: one coset-NTT batch in round 3
+  bytes[kNum] = bytes[kDen] = n * 32;
+  bytes[kW8] = 6 * 8 * n * 32;
+  bytes[kQuot] = bytes[kTcoef] = 8 * n * 32;
+  bytes[kTq] = 4 * stride * 32;
+  bytes[kAgg] = bytes[kPw] = bytes[kScratch] = 2 * stride * 32;
+  bytes[kEvals] = 16 * 32;
+  bytes[kPartial] = (size_t)16 * div_up(stride, 2048) * 32;
+  bytes[kFlag] = 4;
+}
 
 static void compress_affine(const uint64_t* raw, uint8_t out[48]) { pbh::g1_compress_raw(raw, out); }
 
@@ -668,7 +664,7 @@ static int prover_build(pb200_prover* P, const uint8_t* label, size_t label_len,
   P->n8 = 8 * n;
   P->log_n = log_n;
   if (log_n + 3 >= 32) return fail(PB200_ERR_INVALID_DOMAIN, "quotient domain too large");
-  PB_TRY(srs_upload(srs_raw, keep + 1, &P->srs));
+  PB_TRY(srs_upload(srs_raw, keep + 1, &P->srs, 0));
   {
     static const bool lagrange_env = [] {
       const char* e = getenv("PB200_LAGRANGE");
@@ -766,7 +762,7 @@ static int prover_build(pb200_prover* P, const uint8_t* label, size_t label_len,
     // commitments (compiler.rs:213-232): an all-zero selector commits to the identity
     {
       std::vector<uint64_t> aff((size_t)N_POLY * 12);
-      PB_TRY(msm_run(P->srs, 0, (const uint64_t*)P->d_polys, n, N_POLY, n, aff.data(), st, nullptr));
+      PB_TRY(msm_run(P->srs, 0, (const uint64_t*)P->d_polys, n, N_POLY, n, kMsmLatency, aff.data(), st, nullptr));
       for (int k = 0; k < N_POLY; k++) compress_affine(aff.data() + 12 * k, P->comm[k]);
       const int widget_sel[4] = {Q_RANGE, Q_LOGIC, Q_FIXED, Q_VAR};
       for (int w = 0; w < 4; w++) P->has_widget[w] = (P->comm[widget_sel[w]][0] & 0x40) ? 0 : 1;
@@ -825,13 +821,16 @@ static int prover_build(pb200_prover* P, const uint8_t* label, size_t label_len,
   PB_TRY(ntt_run((const uint64_t*)(P->d_polys + 2 * (size_t)S1 * n), n, (uint64_t*)P->d_sigma, log_n, 0, 0, 4, n, n, st, nullptr));
   PB_CUDA(cudaGetLastError());
   PB_CUDA(cudaStreamSynchronize(st));
-  {  // arena size for one proof: prover scratch + the larger of (NTT scratch, MSM scratch)
+  {  // arena of one proof: the buffers prove_dev keeps, then the largest scratch of one call it makes (each call
+     // releases its scratch before the next one carves)
     const size_t stride = n + 8;
-    const size_t elems = 8 * n + 16 * stride + 64 * n + 64 + 16 * (size_t)div_up(stride, 2048) + 4 * (size_t)div_up(stride, 2048);
-    const size_t ntt_tmp = 6 * n8 * 32;
-    size_t msm_ws = msm_workspace_bytes(P->srs, std::min(stride, srs_len(P->srs)), 4);
-    if (P->srs_lag) msm_ws = std::max(msm_ws, msm_workspace_bytes(P->srs_lag, n + 4, 4));
-    P->ws_bytes = elems * 32 + std::max(ntt_tmp, msm_ws) + (size_t)64 * 256 + (1 << 20);
+    size_t call = std::max((size_t)6 * n8 * 32, fr_scan_bytes(stride));  // ntt_run (six polynomials on the 8n coset), fr_scan
+    call = std::max(call, msm_workspace_bytes(P->srs, std::min(stride, srs_len(P->srs)), 4));  // msm_run
+    if (P->srs_lag) call = std::max(call, msm_workspace_bytes(P->srs_lag, n + 4, 4));          // msm_run on the wire values
+    size_t bytes[kProofBufs];
+    proof_buffers(n, bytes);
+    P->ws_bytes = call;
+    for (size_t b : bytes) P->ws_bytes += Arena::round_up(b);
   }
   return 0;
 }
@@ -1128,20 +1127,19 @@ int prove_dev(const pb200_prover* P, int version, const uint64_t* d_wit, const u
               size_t n_pi, const uint64_t* blinders_host, uint8_t* out_proof, cudaStream_t st) {
   const size_t n = P->n, n8 = P->n8, stride = n + 8;
   const int log_n = P->log_n;
-  // With several proofs in flight the dense MSMs give up their latency-oriented bucket splitting (msm.cu)
   struct InFlight {
     const pb200_prover* P;
     explicit InFlight(const pb200_prover* p) : P(p) { P->active.fetch_add(1, std::memory_order_relaxed); }
-    ~InFlight() {
-      P->active.fetch_sub(1, std::memory_order_relaxed);
-      t_msm_throughput_hint = 0;
-      t_msm_wide_heavy_chunks = 0;
-    }
+    ~InFlight() { P->active.fetch_sub(1, std::memory_order_relaxed); }
   } in_flight(P);
-  static const int hint_at = [] {  // PB200_THROUGHPUT_AT=<k>: proofs in flight from which the hint is given (0 = never)
+  static const int hint_at = [] {  // PB200_THROUGHPUT_AT=<k>: proofs in flight from which the prover is busy (0 = never)
     const char* e = getenv("PB200_THROUGHPUT_AT");
     return e ? atoi(e) : 2;
   }();
+  // Busy: other proofs keep the GPU filled, so the MSMs take their throughput shape; `active` changes while this proof
+  // runs, so it is read at each MSM.  Dense scalars then use one lane per bucket and the wide heavy chunks.
+  auto busy = [&] { return hint_at > 0 && (g_force_throughput.load(std::memory_order_relaxed) || P->active.load(std::memory_order_relaxed) >= hint_at); };
+  auto dense_shape = [&] { const bool b = busy(); return MsmShape{!b, b}; };
   const HFr* BL = (const HFr*)blinders_host;
   // the prover's own constraint count stands for VerifierKey::n
   pbh::Transcript tr = version == PB200_PLONK_V3
@@ -1189,25 +1187,16 @@ int prove_dev(const pb200_prover* P, int version, const uint64_t* d_wit, const u
   } release{P, &arena, st};
   Arena* ar = &arena;
   ScratchScope scope(ar, st);
-  uint4 *wv, *wp, *zp, *num, *den, *w8, *quot, *tcoef, *tq, *pi_dense, *agg, *pw, *scratch, *evals_d, *partial;
-  unsigned* flag;
   const unsigned eval_blocks = div_up(stride, 2048);
-  PB_ALLOC(scope, wv, 5 * n * 32);       // wire values a, b, c, d and the dense public-input vector
-  PB_ALLOC(scope, zp, 6 * stride * 32);  // [z, a, b, c, d, pi] coefficient form: one coset-NTT batch in round 3
-  wp = zp + 2 * stride;
-  PB_ALLOC(scope, num, n * 32);
-  PB_ALLOC(scope, den, n * 32);
-  PB_ALLOC(scope, w8, 6 * n8 * 32);
-  PB_ALLOC(scope, quot, n8 * 32);
-  PB_ALLOC(scope, tcoef, n8 * 32);
-  PB_ALLOC(scope, tq, 4 * stride * 32);
-  pi_dense = wv + 2 * 4 * n;
-  PB_ALLOC(scope, agg, 2 * stride * 32);
-  PB_ALLOC(scope, pw, 2 * stride * 32);
-  PB_ALLOC(scope, scratch, 2 * stride * 32);
-  PB_ALLOC(scope, evals_d, 16 * 32);
-  PB_ALLOC(scope, partial, (size_t)16 * eval_blocks * 32);
-  PB_ALLOC(scope, flag, 4);
+  size_t bytes[kProofBufs];
+  void* kept[kProofBufs];
+  proof_buffers(n, bytes);
+  for (int i = 0; i < kProofBufs; i++) PB_ALLOC(scope, kept[i], bytes[i]);
+  uint4 *wv = (uint4*)kept[kWv], *zp = (uint4*)kept[kZp], *num = (uint4*)kept[kNum], *den = (uint4*)kept[kDen], *w8 = (uint4*)kept[kW8],
+        *quot = (uint4*)kept[kQuot], *tcoef = (uint4*)kept[kTcoef], *tq = (uint4*)kept[kTq], *agg = (uint4*)kept[kAgg],
+        *pw = (uint4*)kept[kPw], *scratch = (uint4*)kept[kScratch], *evals_d = (uint4*)kept[kEvals], *partial = (uint4*)kept[kPartial];
+  unsigned* flag = (unsigned*)kept[kFlag];
+  uint4 *wp = zp + 2 * stride, *pi_dense = wv + 2 * 4 * n;
 
   uint64_t aff[4 * 12];
   uint8_t c48[N_COMM][48];
@@ -1242,13 +1231,10 @@ int prove_dev(const pb200_prover* P, int version, const uint64_t* d_wit, const u
     for (int p = 0; p < 4; p++)
       for (int i = 0; i < 2; i++) ba.b[p][i] = to_dev(BL[2 * p + i]);
     PB_LAUNCH(k_lagrange_tail, 1, 32, 0, st, sc, stride, n, ba);
-    t_msm_throughput_hint = 0;  // sparse scalars: long buckets want their lanes
-    t_msm_wide_heavy_chunks = (hint_at > 0 && (g_force_throughput.load(std::memory_order_relaxed) || P->active.load(std::memory_order_relaxed) >= hint_at)) ? 1 : 0;
-    PB_TRY(msm_run(P->srs_lag, 0, (const uint64_t*)sc, n + 4, 4, stride, aff, st, ar));
-    t_msm_wide_heavy_chunks = 0;
+    // sparse scalars: long buckets keep their lanes, only the heavy chunks widen when busy
+    PB_TRY(msm_run(P->srs_lag, 0, (const uint64_t*)sc, n + 4, 4, stride, MsmShape{true, busy()}, aff, st, ar));
   } else {
-    t_msm_throughput_hint = (hint_at > 0 && (g_force_throughput.load(std::memory_order_relaxed) || P->active.load(std::memory_order_relaxed) >= hint_at)) ? 1 : 0;
-    PB_TRY(msm_run(P->srs, 0, (const uint64_t*)wp, n + 2, 4, stride, aff, st, ar));
+    PB_TRY(msm_run(P->srs, 0, (const uint64_t*)wp, n + 2, 4, stride, dense_shape(), aff, st, ar));
   }
   for (int k = 0; k < 4; k++) compress_affine(aff + 12 * k, c48[C_A + k]);
 
@@ -1266,8 +1252,7 @@ int prove_dev(const pb200_prover* P, int version, const uint64_t* d_wit, const u
     for (int i = 0; i < 3; i++) ba.b[0][i] = to_dev(BL[8 + i]);
     PB_LAUNCH(k_blind, 1, 32, 0, st, zp, stride, n, ba);
   }
-  t_msm_throughput_hint = (hint_at > 0 && (g_force_throughput.load(std::memory_order_relaxed) || P->active.load(std::memory_order_relaxed) >= hint_at)) ? 1 : 0;
-  PB_TRY(msm_run(P->srs, 0, (const uint64_t*)zp, n + 3, 1, stride, aff, st, ar));
+  PB_TRY(msm_run(P->srs, 0, (const uint64_t*)zp, n + 3, 1, stride, dense_shape(), aff, st, ar));
   compress_affine(aff, c48[C_Z]);
 
   // ---- round 3 -------------------------------------------------------------------------------
@@ -1373,8 +1358,7 @@ int prove_dev(const pb200_prover* P, int version, const uint64_t* d_wit, const u
   PB_LAUNCH(k_split_quotient, dim3(div_up(stride, 256), 4), 256, 0, st, (const uint4*)tcoef, n, t_len, stride, to_dev(BL[11]), to_dev(BL[12]), to_dev(BL[13]), tq);
   const size_t key_len = srs_len(P->srs);
   const size_t tlen = std::min(stride, key_len);
-  t_msm_throughput_hint = (hint_at > 0 && (g_force_throughput.load(std::memory_order_relaxed) || P->active.load(std::memory_order_relaxed) >= hint_at)) ? 1 : 0;
-  PB_TRY(msm_run(P->srs, 0, (const uint64_t*)tq, tlen, 4, stride, aff, st, ar));  // synchronises the stream
+  PB_TRY(msm_run(P->srs, 0, (const uint64_t*)tq, tlen, 4, stride, dense_shape(), aff, st, ar));  // synchronises the stream
   if (h_flag) return fail(PB200_ERR_UNSATISFIED, "CircuitUnsatisfied");
   for (int k = 0; k < 4; k++) compress_affine(aff + 12 * k, c48[C_T_LOW + k]);
 
@@ -1465,8 +1449,7 @@ int prove_dev(const pb200_prover* P, int version, const uint64_t* d_wit, const u
       PB_LAUNCH(k_mul_pointwise, div_up(stride, 128), 128, 0, st, (const uint4*)c_w, (const uint4*)pw_w, stride, c_w);
     }
     const size_t wlen = std::min(stride, key_len);
-    t_msm_throughput_hint = (hint_at > 0 && (g_force_throughput.load(std::memory_order_relaxed) || P->active.load(std::memory_order_relaxed) >= hint_at)) ? 1 : 0;
-    PB_TRY(msm_run(P->srs, 0, (const uint64_t*)agg, wlen, 2, stride, aff, st, ar));
+    PB_TRY(msm_run(P->srs, 0, (const uint64_t*)agg, wlen, 2, stride, dense_shape(), aff, st, ar));
     compress_affine(aff, c48[C_W_Z]);
     compress_affine(aff + 12, c48[C_W_ZW]);
   }

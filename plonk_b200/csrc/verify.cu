@@ -17,7 +17,7 @@
 #include <thread>
 #include <vector>
 
-#include "common.cuh"
+#include "internal.cuh"
 #include "g1.cuh"
 #include "host_field.h"
 #include "pairing.cuh"
@@ -38,9 +38,6 @@ struct pb200_verifier {
 };
 
 namespace pb {
-void g1_decompress_dev(const uint8_t* d_in, size_t n, uint4* d_out, unsigned* d_bad, cudaStream_t st);
-int g1_decompress(const uint8_t* in, size_t n, int check_subgroup, uint8_t* out_raw);
-
 namespace {
 using pbh::HFr;
 
