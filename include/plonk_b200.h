@@ -25,6 +25,7 @@
  *                                    src/compiler/verifier.rs:32-263
  *   pb200_batch_verify               one verdict for a batch with one pairing, after OpeningKey::batch_check
  *                                    src/commitment_scheme/kzg10/key.rs:571-591, 650-707
+ *   pb200_batch_verify_groups        the same over groups under several verifiers and versions (one SRS)
  *
  * Data layout (identical to the reference's in-memory layout, SURVEY.md section 8):
  *   Fr  (BlsScalar)  4 x u64 little-endian limbs, Montgomery form R = 2^256        -> 32 bytes
@@ -319,6 +320,29 @@ int pb200_batch_verify(const pb200_verifier_t* verifier, int version, const uint
  * layout each, zeros for the identity and when the verdict is decided before the pairing). */
 int pb200_selftest_batch_verify_points(const pb200_verifier_t* verifier, int version, const uint8_t* proofs, size_t n_proofs,
                                        const uint64_t* pi_vals, size_t n_pi, int32_t* verdict, uint8_t* points_2x96);
+/* One verdict for several groups of proofs: group g is n_proofs[g] proofs checked under verifiers[g] and
+ * versions[g], each with n_pi[g] public inputs.  proofs: every group's proofs concatenated in group order
+ * (1008 bytes each); pi_vals: their public inputs concatenated in the same order (Montgomery Fr).
+ * The verifiers may differ (one circuit per group, say) but must share one opening key (the same SRS), since the
+ * folded check e(sum w_i L_i, [x]H) e(sum w_i R_i, H) = 1 has one pairing side; a verifier may appear in several
+ * groups, for example once per version.  rho is drawn as for pb200_batch_verify, except that "version",
+ * "batch-len" and the group's u_i under "batch-u" are appended once per group, in group order; w_i = rho^i over the
+ * proofs in call order.  So one group gives exactly pb200_batch_verify's rho and folded points, and a call holding
+ * an invalid proof passes with probability at most (N - 1) / r over its N proofs.
+ * *verdict: PB200_OK when pb200_verify_with_version(verifiers[g], versions[g], ...) would give PB200_OK to every
+ * proof of every group (up to that bound); otherwise PB200_ERR_POINT_MALFORMED when some proof fails
+ * Proof::from_bytes; otherwise PB200_ERR_VERIFY.  No proofs at all (n_groups = 0, or every group empty) is
+ * PB200_ERR_VERIFY; an empty group among others contributes nothing.  The call fails with PB200_ERR_INVALID_ARG for a
+ * NULL array or verifier, an unknown version, an n_pi[g] that is not verifiers[g]'s public-input count
+ * (InconsistentPublicInputsLen) or verifiers whose OpeningKey::to_bytes differ, and with PB200_ERR_CUDA on a device
+ * failure. */
+int pb200_batch_verify_groups(const pb200_verifier_t* const* verifiers, const int32_t* versions, const size_t* n_proofs,
+                              const size_t* n_pi, size_t n_groups, const uint8_t* proofs, const uint64_t* pi_vals, int32_t* verdict);
+/* Tests only: pb200_batch_verify_groups that also returns the two folded points (the layout of
+ * pb200_selftest_batch_verify_points). */
+int pb200_selftest_batch_verify_groups_points(const pb200_verifier_t* const* verifiers, const int32_t* versions, const size_t* n_proofs,
+                                              const size_t* n_pi, size_t n_groups, const uint8_t* proofs, const uint64_t* pi_vals,
+                                              int32_t* verdict, uint8_t* points_2x96);
 /* Tests only: the device pairing e(P_k, Q_k) for n G1 points (96-byte raw layout) and n compressed G2 points, as
  * Fp12 values of 576 bytes (c0.c0.c0, c0.c0.c1, c0.c1.c0, ..., c1.c2.c1; each Fp 6 x u64 Montgomery limbs). */
 int pb200_selftest_pairing(const uint64_t* g1_raw, const uint8_t* g2_compressed, size_t n, uint64_t* out_fp12);

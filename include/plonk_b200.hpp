@@ -407,6 +407,10 @@ class Prover {
   size_t n_witnesses_;
 };
 
+class Verifier;
+struct BatchGroup;
+inline void batch_verify_groups(const std::vector<BatchGroup>& groups);
+
 // Verifier: verify checks PlonkVersion::V3, verify_with_version any version.  Errors as the reference: verify() throws ProofVerificationError for a proof that
 // fails the check, PointMalformed for one Proof::from_bytes refuses, InvalidArgument for a public-input count that
 // is not the verifier's (InconsistentPublicInputsLen); the constructors throw PointMalformed for a degenerate opening
@@ -489,6 +493,7 @@ class Verifier {
   }
 
  private:
+  friend void batch_verify_groups(const std::vector<BatchGroup>& groups);
   Verifier() = default;
   // the public-input count, read back from Verifier::to_bytes (its fourth big-endian u64)
   size_t pi_count() const {
@@ -504,5 +509,45 @@ class Verifier {
   }
   pb200_verifier_t* h_ = nullptr;
 };
+
+// One group of batch_verify_groups: proofs checked under `verifier` and `version`, with their public inputs.
+struct BatchGroup {
+  const Verifier& verifier;
+  PlonkVersion version;
+  std::vector<std::array<uint8_t, Verifier::PROOF_SIZE>> proofs;
+  std::vector<std::vector<BlsScalar>> public_inputs;
+};
+
+// One verdict for groups of proofs under several verifiers and versions, with one pairing
+// (pb200_batch_verify_groups): returns when every proof would pass its group's verify_with_version (up to a chance of
+// (N - 1) / r over the N proofs); throws PointMalformed when some proof fails Proof::from_bytes, otherwise
+// ProofVerificationError, also when there are no proofs; InvalidArgument for inconsistent public inputs, an unknown
+// version or verifiers with different opening keys.  The verifiers must share one SRS; one may serve several groups.
+inline void batch_verify_groups(const std::vector<BatchGroup>& groups) {
+  std::vector<const pb200_verifier_t*> handles;
+  std::vector<int32_t> versions;
+  std::vector<size_t> n_proofs, n_pi;
+  std::vector<uint8_t> proofs;
+  std::vector<BlsScalar> pi;
+  for (const BatchGroup& g : groups) {
+    if (g.proofs.size() != g.public_inputs.size()) throw Error(Error::InvalidArgument, "one public-input vector per proof");
+    const size_t k = g.public_inputs.empty() ? g.verifier.pi_count() : g.public_inputs[0].size();
+    for (const auto& v : g.public_inputs) {
+      if (v.size() != k) throw Error(Error::InvalidArgument, "every proof needs the same number of public inputs");
+      pi.insert(pi.end(), v.begin(), v.end());
+    }
+    for (const auto& p : g.proofs) proofs.insert(proofs.end(), p.begin(), p.end());
+    handles.push_back(g.verifier.h_);
+    versions.push_back((int32_t)g.version);
+    n_proofs.push_back(g.proofs.size());
+    n_pi.push_back(k);
+  }
+  int32_t verdict = PB200_OK;
+  Verifier::check_verifier(pb200_batch_verify_groups(handles.data(), versions.data(), n_proofs.data(), n_pi.data(), groups.size(),
+                                                     proofs.empty() ? nullptr : proofs.data(), pi.empty() ? nullptr : pi[0].data(),
+                                                     &verdict));
+  if (verdict == PB200_ERR_POINT_MALFORMED) throw Error(Error::PointMalformed, "InvalidData: malformed proof");
+  Verifier::check_verifier(verdict);
+}
 
 }  // namespace plonk_b200

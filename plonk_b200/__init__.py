@@ -10,4 +10,4 @@ from ._lib import Pb200Error, PlonkVersion, lib  # noqa: F401
 from .domain import EvaluationDomain  # noqa: F401
 from .kzg import CommitKey, Commitment, PolynomialDegreeTooLarge  # noqa: F401
 from .prover import CircuitUnsatisfied, Prover, UnsupportedProvingVersion  # noqa: F401
-from .verifier import PointMalformed, ProofVerificationError, Verifier  # noqa: F401
+from .verifier import PointMalformed, ProofVerificationError, Verifier, batch_verify_groups  # noqa: F401

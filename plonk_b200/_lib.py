@@ -46,7 +46,7 @@ EXPORTS = [
     "pb200_prover_new", "pb200_prover_from_bytes", "pb200_prover_free", "pb200_prover_commitments", "pb200_prove", "pb200_prove_dev",
     "pb200_prove_with_version", "pb200_prove_dev_with_version",
     "pb200_verifier_new", "pb200_verifier_from_bytes", "pb200_verifier_to_bytes", "pb200_verifier_free", "pb200_verify", "pb200_verify_with_version",
-    "pb200_batch_verify", "pb200_selftest_batch_verify_points",
+    "pb200_batch_verify", "pb200_selftest_batch_verify_points", "pb200_batch_verify_groups", "pb200_selftest_batch_verify_groups_points",
     "pb200_imad_peak", "pb200_fp_product_peak", "pb200_selftest_pairing", "pb200_selftest_fr_mul", "pb200_selftest_fp_mul", "pb200_selftest_fp_ops",
 ]
 
@@ -141,6 +141,8 @@ def lib() -> ctypes.CDLL:
         L.pb200_verify_with_version.argtypes = [c.c_void_p, c.c_int] + L.pb200_verify.argtypes[1:]
         L.pb200_batch_verify.argtypes = L.pb200_verify_with_version.argtypes
         L.pb200_selftest_batch_verify_points.argtypes = L.pb200_batch_verify.argtypes + [c.c_void_p]
+        L.pb200_batch_verify_groups.argtypes = [c.c_void_p, c.c_void_p, c.c_void_p, c.c_void_p, c.c_size_t, c.c_void_p, c.c_void_p, c.c_void_p]
+        L.pb200_selftest_batch_verify_groups_points.argtypes = L.pb200_batch_verify_groups.argtypes + [c.c_void_p]
         L.pb200_selftest_pairing.argtypes = [c.c_void_p, c.c_void_p, c.c_size_t, c.c_void_p]
         _bind_composer(L)
         _lib = L

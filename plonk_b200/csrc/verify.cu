@@ -8,13 +8,16 @@
 // with one thread per proof (k_verify_pairing).  The device work is the same for every version: V1 only gives the
 // four selector-opening terms zero scalars.
 //
-// Batch verification (pb200_batch_verify) gives one verdict for the whole batch with one pairing: the host draws
-// rho from the batch's u challenges (verify_scalars.h), k_batch_fold weighs each proof's terms by w_i = rho^i and
-// sums the verifier-key terms over the batch, k_batch_msm / k_batch_reduce form sum w_i L_i and sum w_i R_i, and
-// k_verify_pairing checks the pair.
+// Batch verification (pb200_batch_verify_groups, and pb200_batch_verify as its one-group case) gives one verdict for
+// groups of proofs under verifiers that share one opening key, with one pairing: the host draws rho from the groups'
+// versions, lengths and u challenges (verify_scalars.h), k_batch_fold weighs each proof's terms by w_i = rho^i and sums
+// the verifier-key terms per key slot (one slot per distinct verifier), k_batch_msm / k_batch_reduce form
+// sum w_i L_i and sum w_i R_i, and k_verify_pairing checks the pair.
 #include <algorithm>
 #include <mutex>
+#include <numeric>
 #include <thread>
+#include <unordered_map>
 #include <vector>
 
 #include "internal.cuh"
@@ -164,9 +167,15 @@ __global__ void __launch_bounds__(64) k_verify_pairing(const uint4* g1, const Li
 // Proof i's check is e(L_i, [x]H) e(R_i, H) = 1 with L_i = -(W_z + u_i W_zw) and R_i = sum_k s_ik P_ik, the 31 terms
 // of k_verify_msm's lanes 0..30.  The batch's check is the same with L = sum w_i L_i and R = sum w_i R_i, formed as
 // two dense term lists: R has the 11 proof commitments of every proof (term 11 i + j is commitment j of proof i, so
-// its point is pts[11 i + j]) followed by the 16 key points, whose scalars are summed over the batch; L has W_z and
+// its point is pts[11 i + j]) followed by 16 key points per key slot (term 11 n + 16 s + k is key point k of slot s,
+// read from the gathered table key_pts[16 s + k]), whose scalars are summed over the slot's proofs; L has W_z and
 // W_zw of every proof (terms 2 i and 2 i + 1) and is negated once at the end.
 constexpr int kBatchFoldWarps = 8;  // proofs per block of k_batch_fold
+
+// A block of k_batch_fold: proofs [first, first + count), count <= kBatchFoldWarps, all under one key slot.
+struct FoldBlock {
+  uint32_t first, count;
+};
 
 PB_D Fr ld_fr(const uint4* q) {
   Fr x;
@@ -184,16 +193,18 @@ PB_D void st_fr(uint4* q, const Fr& x) {
 // canonical scalar is canonical); status: the host's verdicts.  A proof that the host or the decoder rejected gets
 // weight 0 and sets flags (bit 0: malformed, bit 1: fails the check).  Writes the 11 n proof-term scalars of R
 // (r_scal) and the 2 n scalars of L (l_scal: w_i, w_i u_i), and per block the sums over its proofs of the 19
-// key-point lanes, merged into the 16 key points (key_part: [block][16]).
+// key-point lanes, merged into the 16 key points (key_part: [block][16]).  blocks: which proofs each block takes;
+// the host lists the blocks slot by slot, so that a slot's partial sums are one contiguous range.
 __global__ void __launch_bounds__(32 * kBatchFoldWarps) k_batch_fold(const uint4* pts, const uint8_t* proof_comm, const uint4* scalars,
-                                                                    const uint4* weights, const int* status, size_t n, unsigned* flags,
-                                                                    uint4* r_scal, uint4* l_scal, uint4* key_part) {
+                                                                    const uint4* weights, const int* status, const FoldBlock* blocks,
+                                                                    unsigned* flags, uint4* r_scal, uint4* l_scal, uint4* key_part) {
   __shared__ uint4 part[kBatchFoldWarps][32][2];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const size_t i = (size_t)blockIdx.x * kBatchFoldWarps + warp;
+  const FoldBlock blk = blocks[blockIdx.x];
+  const size_t i = (size_t)blk.first + warp;
   const int src = c_term_point[lane];
   Fr prod = Fr::zero();
-  if (i < n) {  // whole warps
+  if (warp < (int)blk.count) {  // whole warps
     const bool bad = warp_proof_malformed(pts, proof_comm, i, lane);
     const int st = bad ? PB200_ERR_POINT_MALFORMED : status[i];
     if (lane == 0 && st != PB200_OK) atomicOr(flags, st == PB200_ERR_POINT_MALFORMED ? 1u : 2u);
@@ -217,13 +228,15 @@ __global__ void __launch_bounds__(32 * kBatchFoldWarps) k_batch_fold(const uint4
   }
 }
 
-// Block k sums key point k's partial scalars over the n_blocks blocks of k_batch_fold into r_keys[k]; block 0 turns
-// the flags into the verdict (malformed before a failed check).
-__global__ void __launch_bounds__(256) k_batch_key_sums(const uint4* key_part, size_t n_blocks, const unsigned* flags, int* verdict,
-                                                        uint4* r_keys) {
+// Block 16 s + k sums key point k's partial scalars over slot s's blocks of k_batch_fold, [slot_blocks[s],
+// slot_blocks[s + 1]), into r_keys[16 s + k]; block 0 turns the flags into the verdict (malformed before a failed
+// check).
+__global__ void __launch_bounds__(256) k_batch_key_sums(const uint4* key_part, const uint32_t* slot_blocks, const unsigned* flags,
+                                                        int* verdict, uint4* r_keys) {
   __shared__ uint4 s[256][2];
+  const uint32_t slot = blockIdx.x >> 4, k = blockIdx.x & 15;
   Fr acc = Fr::zero();
-  for (size_t b = threadIdx.x; b < n_blocks; b += 256) acc = acc + ld_fr(key_part + 2 * (b * 16 + blockIdx.x));
+  for (size_t b = slot_blocks[slot] + threadIdx.x; b < slot_blocks[slot + 1]; b += 256) acc = acc + ld_fr(key_part + 2 * (b * 16 + k));
   st_fr(s[threadIdx.x], acc);
   __syncthreads();
   for (int d = 128; d >= 1; d >>= 1) {
@@ -236,19 +249,19 @@ __global__ void __launch_bounds__(256) k_batch_key_sums(const uint4* key_part, s
   }
 }
 
-// One lane per term, 32 terms per warp: threads [0, r_pad) take R's n_r terms, threads [r_pad, r_pad + l_pad) take
-// L's n_l terms (both lists padded to whole warps with empty terms).  Per-lane double-and-add in XYZZ as in
-// k_verify_msm, then a warp sum; partial[warp] receives it.  Nothing runs once the verdict is a failure.
-__global__ void __launch_bounds__(128) k_batch_msm(const uint4* key_pts, const uint4* pts, const uint4* r_scal, size_t n_r,
-                                                   size_t r_pad, const uint4* l_scal, size_t n_l, size_t l_pad, const int* verdict,
-                                                   G1Xyzz* partial) {
+// One lane per term, 32 terms per warp: threads [0, r_pad) take R's n_r terms (the first n_proof_terms of them proof
+// commitments, the rest key points), threads [r_pad, r_pad + l_pad) take L's n_l terms (both lists padded to whole
+// warps with empty terms).  Per-lane double-and-add in XYZZ as in k_verify_msm, then a warp sum; partial[warp]
+// receives it.  Nothing runs once the verdict is a failure.
+__global__ void __launch_bounds__(128) k_batch_msm(const uint4* key_pts, const uint4* pts, const uint4* r_scal, size_t n_proof_terms,
+                                                   size_t n_r, size_t r_pad, const uint4* l_scal, size_t n_l, size_t l_pad,
+                                                   const int* verdict, G1Xyzz* partial) {
   const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= r_pad + l_pad || *verdict != PB200_OK) return;  // whole warps
   const bool is_r = t < r_pad;
   const size_t k = is_r ? t : t - r_pad;
   G1Xyzz acc = G1Xyzz::identity();
   if (k < (is_r ? n_r : n_l)) {
-    const size_t n_proof_terms = n_r - 16;
     const G1Affine p = !is_r ? ld_aff(pts + 6 * ((k >> 1) * 11 + (P_WZ - 16) + (k & 1)))
                        : k < n_proof_terms ? ld_aff(pts + 6 * k)
                                            : ld_aff(key_pts + 6 * (k - n_proof_terms));
@@ -435,19 +448,33 @@ int verifier_build(const uint8_t* label, size_t label_len, uint64_t vk_n, uint64
   return 0;
 }
 
-// The host stage of pb200_verify_with_version and pb200_batch_verify: per proof its commitments (comm), the 32
-// scalars of k_verify_msm (scal), the host's verdict (hstat) and, when us is given, its challenge u; spread over
-// threads for large batches.
-void replay(const pb200_verifier* V, int version, const uint8_t* proofs, size_t n_proofs, const uint64_t* pi_vals, size_t n_pi,
-            std::vector<uint64_t>& scal, std::vector<int>& hstat, std::vector<uint8_t>& comm, HFr* us) {
+// Proofs [first, first + n) of a replay: checked under V and version, proof j of the group at proofs + 1008 j with
+// its V->pi_idx.size() public inputs at pi_vals + 4 n_pi j.
+struct ReplayGroup {
+  const pb200_verifier* V;
+  int version;
+  const uint8_t* proofs;
+  const uint64_t* pi_vals;
+  size_t first, n;
+};
+
+// The host stage of pb200_verify_with_version and batch verification, over every group's proofs at once (groups in
+// order, covering [0, n_proofs)): per proof its commitments (comm), the 32 scalars of k_verify_msm (scal), the host's
+// verdict (hstat) and, when us is given, its challenge u; spread over threads for large calls.
+void replay(const std::vector<ReplayGroup>& groups, size_t n_proofs, std::vector<uint64_t>& scal, std::vector<int>& hstat,
+            std::vector<uint8_t>& comm, HFr* us) {
   scal.assign(n_proofs * PB_VERIFY_TERMS * 4, 0);
   hstat.assign(n_proofs, 0);
   comm.assign(n_proofs * kProofEvalAt, 0);
   auto work = [&](size_t lo, size_t hi) {
+    size_t g = 0;
     for (size_t i = lo; i < hi; i++) {
-      const uint8_t* pr = proofs + kProofBytes * i;
+      while (i >= groups[g].first + groups[g].n) g++;
+      const ReplayGroup& G = groups[g];
+      const size_t j = i - G.first, n_pi = G.V->pi_idx.size();
+      const uint8_t* pr = G.proofs + kProofBytes * j;
       memcpy(comm.data() + kProofEvalAt * i, pr, kProofEvalAt);
-      hstat[i] = verify_scalars(V->key, version, pr, (const HFr*)(pi_vals + 4 * n_pi * i), scal.data() + (size_t)PB_VERIFY_TERMS * 4 * i,
+      hstat[i] = verify_scalars(G.V->key, G.version, pr, (const HFr*)(G.pi_vals + 4 * n_pi * j), scal.data() + (size_t)PB_VERIFY_TERMS * 4 * i,
                                 us ? us + i : nullptr);
     }
   };
@@ -462,17 +489,40 @@ void replay(const pb200_verifier* V, int version, const uint8_t* proofs, size_t 
   }
 }
 
-// pb200_batch_verify; points, when given, receives sum w_i L_i then sum w_i R_i (96-byte raw affine each; zeros when
-// the verdict is decided before the pairing).
-int batch_verify(const pb200_verifier_t* V, int version, const uint8_t* proofs, size_t n_proofs, const uint64_t* pi_vals, size_t n_pi,
-                 int32_t* verdict, uint8_t* points) {
+// pb200_batch_verify_groups (pb200_batch_verify is its one-group case); points, when given, receives sum w_i L_i then
+// sum w_i R_i (96-byte raw affine each; zeros when the verdict is decided before the pairing).
+int batch_verify(const pb200_verifier_t* const* Vs, const int32_t* versions, const size_t* n_proofs, const size_t* n_pi, size_t n_groups,
+                 const uint8_t* proofs, const uint64_t* pi_vals, int32_t* verdict, uint8_t* points) {
   PB_TRY(ensure_init());
-  if (!V || (!proofs && n_proofs) || (!pi_vals && n_pi && n_proofs) || !verdict) return fail(PB200_ERR_INVALID_ARG, "null argument");
-  if (version != PB200_PLONK_V1 && version != PB200_PLONK_V2 && version != PB200_PLONK_V3)
-    return fail(PB200_ERR_INVALID_ARG, "unknown PlonkVersion");
-  if (n_pi != V->pi_idx.size()) return fail(PB200_ERR_INVALID_ARG, "InconsistentPublicInputsLen");
+  if (!verdict || (n_groups && (!Vs || !versions || !n_proofs || !n_pi))) return fail(PB200_ERR_INVALID_ARG, "null argument");
+  // the groups in call order, and one key slot per distinct verifier (slots in order of first appearance)
+  std::vector<ReplayGroup> groups(n_groups);
+  std::vector<const pb200_verifier*> slot_v;
+  std::unordered_map<const pb200_verifier*, uint32_t> slot_index;
+  std::vector<uint32_t> slot_of(n_groups);
+  size_t n = 0, n_pi_words = 0;
+  for (size_t g = 0; g < n_groups; g++) {
+    const pb200_verifier* V = Vs[g];
+    if (!V) return fail(PB200_ERR_INVALID_ARG, "null argument");
+    if (versions[g] != PB200_PLONK_V1 && versions[g] != PB200_PLONK_V2 && versions[g] != PB200_PLONK_V3)
+      return fail(PB200_ERR_INVALID_ARG, "unknown PlonkVersion");
+    if (n_pi[g] != V->pi_idx.size()) return fail(PB200_ERR_INVALID_ARG, "InconsistentPublicInputsLen");
+    if (memcmp(V->opening_key, Vs[0]->opening_key, PB200_OPENING_KEY_BYTES))
+      return fail(PB200_ERR_INVALID_ARG, "the verifiers of one batch must share one opening key (one SRS)");
+    const auto slot = slot_index.emplace(V, (uint32_t)slot_v.size());
+    if (slot.second) slot_v.push_back(V);
+    slot_of[g] = slot.first->second;
+    n += n_proofs[g];
+    n_pi_words += 4 * n_pi[g] * n_proofs[g];
+  }
+  if ((!proofs && n) || (!pi_vals && n_pi_words)) return fail(PB200_ERR_INVALID_ARG, "null argument");
+  for (size_t g = 0, first = 0, pi_at = 0; g < n_groups; g++) {
+    groups[g] = {Vs[g], versions[g], proofs ? proofs + kProofBytes * first : nullptr, pi_vals ? pi_vals + pi_at : nullptr, first, n_proofs[g]};
+    first += n_proofs[g];
+    pi_at += 4 * n_pi[g] * n_proofs[g];
+  }
   if (points) memset(points, 0, 2 * 96);
-  if (!n_proofs) {  // batch_check rejects an empty batch (key.rs:667-669)
+  if (!n) {  // batch_check rejects an empty batch (key.rs:667-669)
     *verdict = PB200_ERR_VERIFY;
     return 0;
   }
@@ -480,8 +530,8 @@ int batch_verify(const pb200_verifier_t* V, int version, const uint8_t* proofs, 
   std::vector<uint64_t> scal;
   std::vector<int> hstat;
   std::vector<uint8_t> comm;
-  std::vector<HFr> us(n_proofs);
-  replay(V, version, proofs, n_proofs, pi_vals, n_pi, scal, hstat, comm, us.data());
+  std::vector<HFr> us(n);
+  replay(groups, n, scal, hstat, comm, us.data());
   bool host_ok = true;
   for (int h : hstat) {
     if (h == PB200_ERR_POINT_MALFORMED) {
@@ -492,14 +542,28 @@ int batch_verify(const pb200_verifier_t* V, int version, const uint8_t* proofs, 
   }
   // rho is needed only when every proof passed the host stage; otherwise the verdict is a failure whatever the
   // weights, and the device still looks for malformed commitments, which take precedence
-  const std::vector<HFr> w = host_ok ? batch_weights(batch_challenge(version, us.data(), n_proofs), n_proofs)
-                                     : std::vector<HFr>(n_proofs, HFr::zero());
-  const size_t n = n_proofs, fold_blocks = div_up(n, kBatchFoldWarps);
-  const size_t n_r = 11 * n + 16, r_pad = (n_r + 31) / 32 * 32, n_l = 2 * n, l_pad = (n_l + 31) / 32 * 32;
+  const std::vector<HFr> w = host_ok ? batch_weights(batch_challenge(versions, n_proofs, n_groups, us.data()), n) : std::vector<HFr>(n, HFr::zero());
+  // k_batch_fold's blocks slot by slot: each group's proofs in runs of kBatchFoldWarps, so no block spans two slots
+  // (one group gives blocks {8 b, min(8, n - 8 b)}); slot_blocks[s] is slot s's first block
+  const size_t n_slots = slot_v.size();
+  std::vector<size_t> order(n_groups);
+  std::iota(order.begin(), order.end(), 0);
+  std::stable_sort(order.begin(), order.end(), [&](size_t a, size_t b) { return slot_of[a] < slot_of[b]; });
+  std::vector<FoldBlock> blocks;
+  std::vector<uint32_t> slot_blocks(n_slots + 1, 0);
+  for (size_t g : order) {
+    for (size_t j = 0; j < n_proofs[g]; j += kBatchFoldWarps)
+      blocks.push_back({(uint32_t)(groups[g].first + j), (uint32_t)std::min<size_t>(kBatchFoldWarps, n_proofs[g] - j)});
+    slot_blocks[slot_of[g] + 1] = (uint32_t)blocks.size();
+  }
+  const size_t fold_blocks = blocks.size();
+  const size_t n_r = 11 * n + 16 * n_slots, r_pad = (n_r + 31) / 32 * 32, n_l = 2 * n, l_pad = (n_l + 31) / 32 * 32;
   cudaStream_t st = thread_stream();
   ScratchScope scope(nullptr, st);
   uint8_t* d_comm;
-  uint4 *d_pts, *d_scal, *d_w, *d_rs, *d_ls, *d_keypart, *d_g1;
+  uint4 *d_pts, *d_scal, *d_w, *d_rs, *d_ls, *d_keypart, *d_keypts, *d_g1;
+  FoldBlock* d_blocks;
+  uint32_t* d_slot_blocks;
   G1Xyzz* d_part;
   unsigned *d_bad, *d_flags;
   int *d_stat, *d_verdict;
@@ -510,6 +574,9 @@ int batch_verify(const pb200_verifier_t* V, int version, const uint8_t* proofs, 
   PB_ALLOC(scope, d_rs, n_r * 32);
   PB_ALLOC(scope, d_ls, n_l * 32);
   PB_ALLOC(scope, d_keypart, fold_blocks * 16 * 32);
+  PB_ALLOC(scope, d_keypts, n_slots * 16 * 96);
+  PB_ALLOC(scope, d_blocks, fold_blocks * sizeof(FoldBlock));
+  PB_ALLOC(scope, d_slot_blocks, slot_blocks.size() * sizeof(uint32_t));
   PB_ALLOC(scope, d_part, (r_pad + l_pad) / 32 * sizeof(G1Xyzz));
   PB_ALLOC(scope, d_g1, 2 * 96);
   PB_ALLOC(scope, d_bad, 4);
@@ -521,14 +588,20 @@ int batch_verify(const pb200_verifier_t* V, int version, const uint8_t* proofs, 
   PB_CUDA(cudaMemcpyAsync(d_scal, scal.data(), scal.size() * 8, cudaMemcpyHostToDevice, st));
   PB_CUDA(cudaMemcpyAsync(d_w, w.data(), n * 32, cudaMemcpyHostToDevice, st));
   PB_CUDA(cudaMemcpyAsync(d_stat, hstat.data(), n * sizeof(int), cudaMemcpyHostToDevice, st));
+  PB_CUDA(cudaMemcpyAsync(d_blocks, blocks.data(), fold_blocks * sizeof(FoldBlock), cudaMemcpyHostToDevice, st));
+  PB_CUDA(cudaMemcpyAsync(d_slot_blocks, slot_blocks.data(), slot_blocks.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+  for (size_t s = 0; s < n_slots; s++)  // each slot's 16 key points: the 15 commitments, then opening_key.g
+    PB_CUDA(cudaMemcpyAsync(d_keypts + 16 * 6 * s, slot_v[s]->d_points, 16 * 96, cudaMemcpyDeviceToDevice, st));
   PB_CUDA(cudaMemsetAsync(d_flags, 0, 4, st));
   PB_CUDA(cudaMemsetAsync(d_g1, 0, 2 * 96, st));
   g1_decompress_dev(d_comm, n * 11, d_pts, d_bad, st);
-  PB_LAUNCH(k_batch_fold, fold_blocks, 32 * kBatchFoldWarps, 0, st, d_pts, d_comm, d_scal, d_w, d_stat, n, d_flags, d_rs, d_ls, d_keypart);
-  PB_LAUNCH(k_batch_key_sums, 16, 256, 0, st, d_keypart, fold_blocks, d_flags, d_verdict, d_rs + 2 * 11 * n);
-  PB_LAUNCH(k_batch_msm, div_up(r_pad + l_pad, 128), 128, 0, st, V->d_points, d_pts, d_rs, n_r, r_pad, d_ls, n_l, l_pad, d_verdict, d_part);
+  PB_LAUNCH(k_batch_fold, fold_blocks, 32 * kBatchFoldWarps, 0, st, d_pts, d_comm, d_scal, d_w, d_stat, d_blocks, d_flags, d_rs, d_ls, d_keypart);
+  PB_LAUNCH(k_batch_key_sums, 16 * n_slots, 256, 0, st, d_keypart, d_slot_blocks, d_flags, d_verdict, d_rs + 2 * 11 * n);
+  PB_LAUNCH(k_batch_msm, div_up(r_pad + l_pad, 128), 128, 0, st, d_keypts, d_pts, d_rs, 11 * n, n_r, r_pad, d_ls, n_l, l_pad, d_verdict,
+            d_part);
   PB_LAUNCH(k_batch_reduce, 2, 256, 0, st, d_part, r_pad / 32, l_pad / 32, d_verdict, d_g1);
-  PB_LAUNCH(k_verify_pairing, 1, 64, 0, st, d_g1, V->d_lines, 1, d_verdict);
+  // the verifiers share their opening key, so the first one's prepared [x]H and H serve the whole call
+  PB_LAUNCH(k_verify_pairing, 1, 64, 0, st, d_g1, Vs[0]->d_lines, 1, d_verdict);
   PB_CUDA(cudaGetLastError());
   int v = 0;
   PB_CUDA(cudaMemcpyAsync(&v, d_verdict, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -633,7 +706,7 @@ int pb200_verify_with_version(const pb200_verifier_t* V, int version, const uint
   std::vector<uint64_t> scal;
   std::vector<int> hstat;
   std::vector<uint8_t> comm;
-  replay(V, version, proofs, n_proofs, pi_vals, n_pi, scal, hstat, comm, nullptr);
+  replay({{V, version, proofs, pi_vals, 0, n_proofs}}, n_proofs, scal, hstat, comm, nullptr);
   // device: decoding, the two G1 points, the pairing check
   cudaStream_t st = thread_stream();
   ScratchScope scope(nullptr, st);
@@ -662,13 +735,25 @@ int pb200_verify_with_version(const pb200_verifier_t* V, int version, const uint
 
 int pb200_batch_verify(const pb200_verifier_t* V, int version, const uint8_t* proofs, size_t n_proofs, const uint64_t* pi_vals,
                        size_t n_pi, int32_t* verdict) {
-  return batch_verify(V, version, proofs, n_proofs, pi_vals, n_pi, verdict, nullptr);
+  return batch_verify(&V, &version, &n_proofs, &n_pi, 1, proofs, pi_vals, verdict, nullptr);
 }
 
 int pb200_selftest_batch_verify_points(const pb200_verifier_t* V, int version, const uint8_t* proofs, size_t n_proofs,
                                        const uint64_t* pi_vals, size_t n_pi, int32_t* verdict, uint8_t* points_2x96) {
   if (!points_2x96) return fail(PB200_ERR_INVALID_ARG, "null argument");
-  return batch_verify(V, version, proofs, n_proofs, pi_vals, n_pi, verdict, points_2x96);
+  return batch_verify(&V, &version, &n_proofs, &n_pi, 1, proofs, pi_vals, verdict, points_2x96);
+}
+
+int pb200_batch_verify_groups(const pb200_verifier_t* const* verifiers, const int32_t* versions, const size_t* n_proofs,
+                              const size_t* n_pi, size_t n_groups, const uint8_t* proofs, const uint64_t* pi_vals, int32_t* verdict) {
+  return batch_verify(verifiers, versions, n_proofs, n_pi, n_groups, proofs, pi_vals, verdict, nullptr);
+}
+
+int pb200_selftest_batch_verify_groups_points(const pb200_verifier_t* const* verifiers, const int32_t* versions, const size_t* n_proofs,
+                                              const size_t* n_pi, size_t n_groups, const uint8_t* proofs, const uint64_t* pi_vals,
+                                              int32_t* verdict, uint8_t* points_2x96) {
+  if (!points_2x96) return fail(PB200_ERR_INVALID_ARG, "null argument");
+  return batch_verify(verifiers, versions, n_proofs, n_pi, n_groups, proofs, pi_vals, verdict, points_2x96);
 }
 
 int pb200_selftest_pairing(const uint64_t* g1_raw, const uint8_t* g2_compressed, size_t n, uint64_t* out_fp12) {

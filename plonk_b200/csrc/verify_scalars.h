@@ -138,14 +138,22 @@ inline int verify_scalars(const VerifyKeyHost& K, int version, const uint8_t* pr
 // challenge, from a transcript over the whole batch: the version, the length and each proof's u in batch order.  u
 // is the last Fiat-Shamir challenge of its proof, so it binds the key, the seed, the public inputs and every proof
 // byte, and rho is fixed only once the whole batch is.  us: Montgomery form; returns rho in Montgomery form.
-inline pbh::HFr batch_challenge(int version, const pbh::HFr* us, size_t n) {
+//
+// A call over several groups (group g: lens[g] proofs under versions[g], each group under its own verifier) appends
+// "version", "batch-len" and the group's u values once per group, in call order, so one group draws exactly the rho
+// above.  u binds its proof's verifier key, but not V1 against V2 (both start from the legacy seed), hence the
+// per-group version; the per-group lengths make the sequence parse one way only.  us: every group's u in call order.
+inline pbh::HFr batch_challenge(const int* versions, const size_t* lens, size_t n_groups, const pbh::HFr* us) {
   pbh::Transcript t((const uint8_t*)"dusk-plonk", 10);
   t.append_message("dom-sep", (const uint8_t*)"plonk-batch-verify-v1", 21);
-  t.append_u64("version", (uint64_t)version);
-  t.append_u64("batch-len", (uint64_t)n);
-  for (size_t i = 0; i < n; i++) t.append_scalar("batch-u", us[i]);
+  for (size_t g = 0; g < n_groups; g++) {
+    t.append_u64("version", (uint64_t)versions[g]);
+    t.append_u64("batch-len", (uint64_t)lens[g]);
+    for (size_t i = 0; i < lens[g]; i++) t.append_scalar("batch-u", *us++);
+  }
   return t.challenge_scalar("batch-challenge");
 }
+inline pbh::HFr batch_challenge(int version, const pbh::HFr* us, size_t n) { return batch_challenge(&version, &n, 1, us); }
 
 // w_i = rho^i for i = 0 .. n-1 (Montgomery form).
 inline std::vector<pbh::HFr> batch_weights(const pbh::HFr& rho, size_t n) {

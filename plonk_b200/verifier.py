@@ -1,9 +1,10 @@
-"""Verifier (reference src/compiler/verifier.rs) on the GPU, through pb200_verifier_*, pb200_verify_with_version and
-pb200_batch_verify of include/plonk_b200.h.  Every PlonkVersion is verified on the device; V3 is the default."""
+"""Verifier (reference src/compiler/verifier.rs) on the GPU, through pb200_verifier_*, pb200_verify_with_version,
+pb200_batch_verify and pb200_batch_verify_groups of include/plonk_b200.h.  Every PlonkVersion is verified on the
+device; V3 is the default."""
 from __future__ import annotations
 
 import ctypes
-from typing import List, Sequence
+from typing import List, Sequence, Tuple
 
 from ._lib import PB200_ERR_INVALID_ARG, PB200_ERR_POINT_MALFORMED, PB200_ERR_VERIFY, Pb200Error, PlonkVersion, check, lib
 
@@ -71,17 +72,8 @@ class Verifier:
             raise ValueError("every proof needs the same number of public inputs")
         verdict = ctypes.c_int32()
         vals = b"".join(pi_vals)
-        try:
-            check(lib().pb200_batch_verify(self._h, int(version), b"".join(proofs) or None, len(proofs), vals or None, n_pi,
-                                           ctypes.byref(verdict)))
-        except Pb200Error as e:
-            if e.code == PB200_ERR_INVALID_ARG:
-                raise ValueError(str(e)) from e
-            raise
-        if verdict.value == PB200_ERR_VERIFY:
-            raise ProofVerificationError("ProofVerificationError")
-        if verdict.value == PB200_ERR_POINT_MALFORMED:
-            raise PointMalformed("InvalidData")
+        _raise_verdict(lambda: lib().pb200_batch_verify(self._h, int(version), b"".join(proofs) or None, len(proofs), vals or None,
+                                                        n_pi, ctypes.byref(verdict)), verdict)
 
     def verify(self, proof: bytes, pi_vals: bytes) -> None:
         """Verifier::verify: returns on success, raises ProofVerificationError, PointMalformed or ValueError."""
@@ -108,3 +100,45 @@ class Verifier:
                 self._h = None
         except Exception:
             pass
+
+
+def _raise_verdict(call, verdict: ctypes.c_int32) -> None:
+    """Runs a batch call and turns its return code and verdict into the errors of Verifier.batch_verify."""
+    try:
+        check(call())
+    except Pb200Error as e:
+        if e.code == PB200_ERR_INVALID_ARG:
+            raise ValueError(str(e)) from e
+        raise
+    if verdict.value == PB200_ERR_VERIFY:
+        raise ProofVerificationError("ProofVerificationError")
+    if verdict.value == PB200_ERR_POINT_MALFORMED:
+        raise PointMalformed("InvalidData")
+
+
+def batch_verify_groups(groups: Sequence[Tuple[Verifier, Sequence[bytes], Sequence[bytes], PlonkVersion]]) -> None:
+    """One verdict for groups of proofs under several verifiers and versions, at the cost of one pairing
+    (pb200_batch_verify_groups).  groups: (verifier, proofs, pi_vals, version) each, as Verifier.batch_verify takes
+    them; the verifiers must share one opening key (one SRS), and one verifier may appear in several groups.  Returns
+    when every proof would pass its group's verify_with_version (up to a chance of (N - 1) / r over the N proofs),
+    raises PointMalformed when some proof fails Proof::from_bytes, otherwise ProofVerificationError, also when there
+    are no proofs at all; ValueError for inconsistent public inputs, an unknown version or verifiers with different
+    opening keys."""
+    n_pi, n_proofs, proofs, vals = [], [], [], []
+    for verifier, ps, pis, _ in groups:
+        assert len(ps) == len(pis) and all(len(p) == PROOF_BYTES for p in ps)
+        k = len(pis[0]) // 32 if pis else verifier.n_pi
+        if any(len(v) != 32 * k for v in pis):
+            raise ValueError("every proof needs the same number of public inputs")
+        n_pi.append(k)
+        n_proofs.append(len(ps))
+        proofs += ps
+        vals += pis
+    m = len(groups)
+    handles = (ctypes.c_void_p * max(1, m))(*[g[0]._h.value for g in groups])
+    versions = (ctypes.c_int32 * max(1, m))(*[int(g[3]) for g in groups])
+    counts = (ctypes.c_size_t * max(1, m))(*n_proofs)
+    pi_counts = (ctypes.c_size_t * max(1, m))(*n_pi)
+    verdict = ctypes.c_int32()
+    _raise_verdict(lambda: lib().pb200_batch_verify_groups(handles, versions, counts, pi_counts, m, b"".join(proofs) or None,
+                                                           b"".join(vals) or None, ctypes.byref(verdict)), verdict)
