@@ -26,6 +26,10 @@
  *   pb200_batch_verify               one verdict for a batch with one pairing, after OpeningKey::batch_check
  *                                    src/commitment_scheme/kzg10/key.rs:571-591, 650-707
  *   pb200_batch_verify_groups        the same over groups under several verifiers and versions (one SRS)
+ *   pb200_public_parameters_setup    PublicParameters::setup      src/commitment_scheme/kzg10/srs.rs:61-100
+ *   pb200_opening_key_check          OpeningKey::from_bytes       src/commitment_scheme/kzg10/key.rs:609-648
+ *   (Compiler::compile, src/compiler.rs:116-461, is pb200_prover_new, pb200_prover_commitments and pb200_verifier_new
+ *    in sequence; the mirrors write it once.)
  *
  * Data layout (identical to the reference's in-memory layout, SURVEY.md section 8):
  *   Fr  (BlsScalar)  4 x u64 little-endian limbs, Montgomery form R = 2^256        -> 32 bytes
@@ -62,7 +66,8 @@ typedef enum {
   PB200_ERR_POINT_MALFORMED = -10,/* dusk_bytes::Error::InvalidData / Error::PointMalformed: a G1 encoding that is
                                      not canonical, not on the curve or not in the prime-order subgroup */
   PB200_ERR_VERIFY = -11,         /* Error::ProofVerificationError: the proof does not satisfy the verifier */
-  PB200_ERR_UNSUPPORTED_VERSION = -12 /* Error::UnsupportedProvingVersion: PlonkVersion::V1 proofs cannot be made */
+  PB200_ERR_UNSUPPORTED_VERSION = -12,/* Error::UnsupportedProvingVersion: PlonkVersion::V1 proofs cannot be made */
+  PB200_ERR_DEGREE_IS_ZERO = -13  /* Error::DegreeIsZero: PublicParameters::setup with max_degree = 0 (srs.rs:65-68) */
 } pb200_status;
 
 /* PlonkVersion (src/compiler.rs:22-42), for the *_with_version calls.  V3 is the current profile and the one the
@@ -153,8 +158,22 @@ int pb200_msm_g1_allgather_dev(const pb200_srs_t* srs_slice, const uint64_t* d_s
 int pb200_msm_combine_parts(const uint32_t* parts, int n_parts, int window_bits, uint32_t batch,
                             uint64_t* out_affine, size_t* words_per_entry);
 
-/* PublicParameters::setup with explicit secrets (srs.rs:61-100): out[i] = [g_scalar * x^i] G1, as
- * n_points x 96-byte raw points.  Test/bench helper - a real SRS comes from a ceremony. */
+/* PublicParameters::setup (srs.rs:61-100).  The RNG belongs to the caller, as for pb200_prove's blinders: x, g_scalar and
+ * h_scalar are the three util::random_nonzero_bls_scalar draws in the reference's order (x, then random_g1_point's scalar,
+ * then random_g2_point's; util.rs:50-72), Montgomery form.  Writes max_degree + 7 raw points (max_degree +
+ * ADDED_BLINDING_DEGREE + 1: out_raw_points[i] = [g_scalar * x^i] G1) and OpeningKey::to_bytes (PB200_OPENING_KEY_BYTES:
+ * g = point 0 compressed, h = [h_scalar] G2 and [x] h, compressed G2 points).  The commit key is computed on the GPU by
+ * fixed-base multiplication of the generator (a window table built once per process), the G2 points by one device
+ * thread.  max_degree = 0 is PB200_ERR_DEGREE_IS_ZERO (Error::DegreeIsZero); a NULL pointer, a zero draw or one that is
+ * not below r is PB200_ERR_INVALID_ARG; both are reported before any device is touched. */
+int pb200_public_parameters_setup(size_t max_degree, const uint64_t* x, const uint64_t* g_scalar, const uint64_t* h_scalar,
+                                  uint8_t* out_raw_points, uint8_t* out_opening_key);
+/* OpeningKey::from_bytes (key.rs:609-648) on its own: g, h and [x]h decoded with the on-curve and subgroup checks, the
+ * identity refused (OpeningKey::try_new).  PB200_OK or PB200_ERR_POINT_MALFORMED; NULL is PB200_ERR_INVALID_ARG.
+ * pb200_verifier_new and pb200_verifier_from_bytes apply the same check to their opening key. */
+int pb200_opening_key_check(const uint8_t* opening_key);
+/* The commit-key half of pb200_public_parameters_setup with explicit secrets: out[i] = [g_scalar * x^i] G1, as
+ * n_points x 96-byte raw points (the same kernel). */
 int pb200_srs_setup_from_secret(const uint64_t* x, const uint64_t* g_scalar, size_t n_points,
                                 uint8_t* out_raw);
 

@@ -12,6 +12,9 @@
 //   plonk_b200::Verifier           src/compiler/verifier.rs:32-263                     verify, verify_with_version, to_bytes,
 //                                                                                      try_from_bytes
 //   plonk_b200::PlonkVersion       src/compiler.rs:22-42
+//   plonk_b200::PublicParameters   src/commitment_scheme/kzg10/srs.rs:61-196           setup, from_slice, from_slice_unchecked,
+//                                                                                      to_var_bytes, to_raw_var_bytes, max_degree
+//   plonk_b200::Compiler           src/compiler.rs:47-113, 116-461                     compile, compile_with_circuit
 //   plonk_b200::Composer           src/composer.rs:72-495 + src/composer/{bits,range,logic,truncate,select,
 //                                  point,fixed_base}.rs (host-side circuit front end, plonk_b200_composer.h)
 //   plonk_b200::Error              src/error.rs:21-120 (the variants this path can produce)
@@ -20,11 +23,13 @@
 // Infallible reference functions (the NTT family asserts/panics, domain.rs:394) throw
 // BackendFailure on a device error - there is no CPU fallback.
 #pragma once
+#include <algorithm>
 #include <array>
 #include <cstdint>
 #include <stdexcept>
 #include <memory>
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "plonk_b200.h"
@@ -40,7 +45,10 @@ struct Error : std::runtime_error {
     JubJubPointNotTorsionFree, JubJubGeneratorNotPrimeOrder, JubJubScalarMalformed,
     ProofVerificationError,    // Error::ProofVerificationError
     PointMalformed,            // Error::BytesError(dusk_bytes::Error::InvalidData) of the verifier's decoders
-    UnsupportedProvingVersion  // Error::UnsupportedProvingVersion
+    UnsupportedProvingVersion, // Error::UnsupportedProvingVersion
+    DegreeIsZero,              // Error::DegreeIsZero: PublicParameters::setup with max_degree = 0
+    TruncatedDegreeTooLarge,   // Error::TruncatedDegreeTooLarge: Compiler::compile with too small public parameters
+    NotEnoughBytes             // Error::NotEnoughBytes: PublicParameters::from_slice of at most OpeningKey::SIZE bytes
   };
   Kind kind;
   Error(Kind k, const std::string& what) : std::runtime_error(what), kind(k) {}
@@ -58,6 +66,7 @@ inline void check(int rc) {
     case PB200_ERR_JUBJUB_GENERATOR: throw Error(Error::JubJubGeneratorNotPrimeOrder, msg);
     case PB200_ERR_JUBJUB_SCALAR: throw Error(Error::JubJubScalarMalformed, msg);
     case PB200_ERR_UNSUPPORTED_VERSION: throw Error(Error::UnsupportedProvingVersion, msg);
+    case PB200_ERR_DEGREE_IS_ZERO: throw Error(Error::DegreeIsZero, msg);
     default: throw Error(Error::BackendFailure, msg);
   }
 }
@@ -380,6 +389,7 @@ class Prover {
     return out;
   }
   ~Prover() { pb200_prover_free(h_); }
+  const pb200_prover_t* handle() const { return h_; }
   Prover(const Prover&) = delete;
   Prover& operator=(const Prover&) = delete;
   // Prover::prove: `blinders` are the 14 BlsScalar::random draws of prove_inner, in its order.
@@ -549,5 +559,104 @@ inline void batch_verify_groups(const std::vector<BatchGroup>& groups) {
   if (verdict == PB200_ERR_POINT_MALFORMED) throw Error(Error::PointMalformed, "InvalidData: malformed proof");
   Verifier::check_verifier(verdict);
 }
+
+// PublicParameters (srs.rs): the commit key as 96-byte raw points and OpeningKey::to_bytes.  setup takes the three
+// util::random_nonzero_bls_scalar draws (x, the G1 scalar, the G2 scalar; Montgomery form): the RNG is the caller's.
+// Errors: DegreeIsZero (setup), NotEnoughBytes (from_slice of at most OpeningKey::SIZE bytes), PointMalformed (an
+// invalid opening key, or a commit-key point from_slice refuses), InvalidArgument (a zero draw).
+class PublicParameters {
+ public:
+  static constexpr size_t ADDED_BLINDING_DEGREE = 6;
+  static constexpr size_t OPENING_KEY_SIZE = PB200_OPENING_KEY_BYTES;
+  static std::unique_ptr<PublicParameters> setup(size_t max_degree, const BlsScalar& x, const BlsScalar& g_scalar, const BlsScalar& h_scalar) {
+    std::unique_ptr<PublicParameters> pp(new PublicParameters());
+    pp->raw_.resize(96 * (max_degree + ADDED_BLINDING_DEGREE + 1));
+    check(pb200_public_parameters_setup(max_degree, x.data(), g_scalar.data(), h_scalar.data(), pp->raw_.data(), pp->opening_key_.data()));
+    return pp;
+  }
+  // PublicParameters::from_slice (srs.rs:163-178): the opening key and every commit-key point validated
+  static std::unique_ptr<PublicParameters> from_slice(const uint8_t* bytes, size_t len) {
+    if (len <= OPENING_KEY_SIZE) throw Error(Error::NotEnoughBytes, "NotEnoughBytes");
+    if ((len - OPENING_KEY_SIZE) % 48) throw Error(Error::PointMalformed, "InvalidData: the commit key is not whole 48-byte points");
+    std::unique_ptr<PublicParameters> pp(new PublicParameters());
+    check_points(pb200_opening_key_check(bytes));
+    std::copy(bytes, bytes + OPENING_KEY_SIZE, pp->opening_key_.begin());
+    const size_t n = (len - OPENING_KEY_SIZE) / 48;
+    pp->raw_.resize(96 * n);
+    check_points(pb200_g1_decompress(bytes + OPENING_KEY_SIZE, n, 1, pp->raw_.data()));
+    return pp;
+  }
+  // PublicParameters::from_slice_unchecked (srs.rs:121-146) for to_raw_var_bytes: the opening key validated (the
+  // reference panics where this throws PointMalformed), the commit-key points not
+  static std::unique_ptr<PublicParameters> from_slice_unchecked(const uint8_t* bytes, size_t len) {
+    if (len < OPENING_KEY_SIZE) throw Error(Error::NotEnoughBytes, "NotEnoughBytes");
+    std::unique_ptr<PublicParameters> pp(new PublicParameters());
+    check_points(pb200_opening_key_check(bytes));
+    std::copy(bytes, bytes + OPENING_KEY_SIZE, pp->opening_key_.begin());
+    size_t n = 0;
+    check(pb200_raw_commit_key_points(bytes + OPENING_KEY_SIZE, len - OPENING_KEY_SIZE, 0, &n));
+    pp->raw_.resize(96 * n + 1);
+    check(pb200_commit_key_from_raw_var_bytes(bytes + OPENING_KEY_SIZE, len - OPENING_KEY_SIZE, 0, pp->raw_.data()));
+    pp->raw_.resize(96 * n);
+    return pp;
+  }
+  std::vector<uint8_t> to_var_bytes() const {  // srs.rs:149-153
+    std::vector<uint8_t> out(opening_key_.begin(), opening_key_.end());
+    out.resize(OPENING_KEY_SIZE + 48 * points());
+    check(pb200_g1_compress_batch(raw_.data(), points(), out.data() + OPENING_KEY_SIZE));
+    return out;
+  }
+  std::vector<uint8_t> to_raw_var_bytes() const {  // srs.rs:114-119
+    size_t n = 0;
+    check(pb200_commit_key_to_raw_var_bytes(raw_.data(), points(), nullptr, 0, &n));
+    std::vector<uint8_t> out(opening_key_.begin(), opening_key_.end());
+    out.resize(OPENING_KEY_SIZE + n);
+    check(pb200_commit_key_to_raw_var_bytes(raw_.data(), points(), out.data() + OPENING_KEY_SIZE, n, &n));
+    return out;
+  }
+  size_t max_degree() const { return points() - 1; }
+  std::unique_ptr<CommitKey> commit_key() const { return std::unique_ptr<CommitKey>(new CommitKey(raw_.data(), points())); }
+  const std::array<uint8_t, OPENING_KEY_SIZE>& opening_key() const { return opening_key_; }
+  const std::vector<uint8_t>& raw_points() const { return raw_; }
+  size_t points() const { return raw_.size() / 96; }
+
+ private:
+  PublicParameters() = default;
+  static void check_points(int rc) {
+    if (rc == PB200_ERR_POINT_MALFORMED) throw Error(Error::PointMalformed, std::string("InvalidData: ") + pb200_last_error());
+    check(rc);
+  }
+  std::vector<uint8_t> raw_;
+  std::array<uint8_t, OPENING_KEY_SIZE> opening_key_{};
+};
+
+// Compiler (compiler.rs): Prover::new, the prover's 15 verifier-key commitments and the Verifier over the same opening
+// key.  Public parameters too small for the circuit (pp.max_degree() < next_pow2(constraints + 6) + 6) throw
+// TruncatedDegreeTooLarge.
+struct Compiler {
+  using Pair = std::pair<std::unique_ptr<Prover>, std::unique_ptr<Verifier>>;
+  // Compiler::compile for a filled composer
+  static Pair compile(const PublicParameters& pp, const std::string& label, const Composer& composer) {
+    const Composer::Export e = composer.finish();
+    Pair out;
+    try {
+      out.first.reset(new Prover(label, circuit_of(e), pp.raw_points().data(), pp.points()));
+    } catch (const Error& err) {
+      if (err.kind == Error::PolynomialDegreeTooLarge) throw Error(Error::TruncatedDegreeTooLarge, err.what());
+      throw;
+    }
+    std::array<uint8_t, 15 * 48> comms;
+    check(pb200_prover_commitments(out.first->handle(), comms.data()));
+    out.second.reset(new Verifier(label, e.n_constraints, comms, pp.opening_key(), e.pi_idx));
+    return out;
+  }
+  // Compiler::compile_with_circuit: circuit(composer) fills a fresh Composer::initialized()
+  template <class F>
+  static Pair compile_with_circuit(const PublicParameters& pp, const std::string& label, F&& circuit) {
+    Composer composer;
+    circuit(composer);
+    return compile(pp, label, composer);
+  }
+};
 
 }  // namespace plonk_b200

@@ -20,6 +20,7 @@ PB200_ERR_UNSATISFIED = -5
 PB200_ERR_POINT_MALFORMED = -10
 PB200_ERR_VERIFY = -11
 PB200_ERR_UNSUPPORTED_VERSION = -12
+PB200_ERR_DEGREE_IS_ZERO = -13
 
 
 class PlonkVersion(enum.IntEnum):
@@ -42,6 +43,7 @@ EXPORTS = [
     "pb200_msm_g1", "pb200_msm_g1_dev", "pb200_msm_g1_range", "pb200_msm_g1_allgather", "pb200_msm_g1_allgather_dev", "pb200_msm_combine_parts",
     "pb200_g1_compress", "pb200_g1_compress_batch", "pb200_g1_decompress", "pb200_raw_commit_key_points", "pb200_commit_key_from_raw_var_bytes",
     "pb200_commit_key_to_raw_var_bytes", "pb200_prover_to_bytes", "pb200_g1_add_affine", "pb200_srs_setup_from_secret", "pb200_g1_lagrange_key",
+    "pb200_public_parameters_setup", "pb200_opening_key_check",
     "pb200_profile_enable", "pb200_throughput_mode", "pb200_profile_read", "pb200_profile_read_sparse",
     "pb200_prover_new", "pb200_prover_from_bytes", "pb200_prover_free", "pb200_prover_commitments", "pb200_prove", "pb200_prove_dev",
     "pb200_prove_with_version", "pb200_prove_dev_with_version",
@@ -124,6 +126,8 @@ def lib() -> ctypes.CDLL:
         L.pb200_prove_with_version.argtypes = L.pb200_prove.argtypes[:1] + [c.c_int] + L.pb200_prove.argtypes[1:]
         L.pb200_prove_dev_with_version.argtypes = L.pb200_prove_dev.argtypes[:1] + [c.c_int] + L.pb200_prove_dev.argtypes[1:]
         L.pb200_srs_setup_from_secret.argtypes = [c.c_void_p, c.c_void_p, c.c_size_t, c.c_void_p]
+        L.pb200_public_parameters_setup.argtypes = [c.c_size_t, c.c_void_p, c.c_void_p, c.c_void_p, c.c_void_p, c.c_void_p]
+        L.pb200_opening_key_check.argtypes = [c.c_void_p]
         L.pb200_profile_enable.argtypes = [c.c_int]
         L.pb200_throughput_mode.argtypes = [c.c_int]
         L.pb200_profile_read.argtypes = [c.POINTER(c.c_double), c.POINTER(c.c_uint64), c.POINTER(c.c_uint64), c.POINTER(c.c_uint64)]

@@ -52,6 +52,10 @@ extern std::atomic<uint64_t> g_prof_sp_ns, g_prof_sp_adds, g_prof_sp_launches, g
 // ecntt.cu
 int lagrange_key_dev(const uint4* d_in, int log_n, uint4* d_out, cudaStream_t st);
 
+// verify.cu: OpeningKey::from_bytes's checks alone, and the G2 half of PublicParameters::setup (h, then [x]h, compressed)
+int opening_key_check(const uint8_t* opening_key);
+int opening_key_g2(const uint64_t* x_mont, const uint64_t* h_scalar_mont, uint8_t* out_2x96);
+
 // capi.cu
 int raw_commit_key_parse(const uint8_t* bytes, size_t len, int checked, size_t* n_points, uint8_t* out_raw);
 void raw_commit_key_record(const uint8_t* raw96, uint8_t* rec97);

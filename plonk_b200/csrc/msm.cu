@@ -23,6 +23,7 @@
 //     (Prover::commit_polynomials commits 4 polynomials at once, src/compiler/prover.rs:187-210).
 #include <algorithm>
 #include <atomic>
+#include <mutex>
 #include <vector>
 
 #include "internal.cuh"
@@ -114,31 +115,91 @@ __global__ void k_msm_precompute(uint4* table, size_t n, int c, int W) {
 }
 
 // PublicParameters::setup restated for the device (reference src/commitment_scheme/kzg10/srs.rs:61-100):
-// out[i] = [g_scalar * x^i] G1::generator, normalised to affine.  One thread per power.
-__global__ void __launch_bounds__(64) k_srs_setup(uint4* out, size_t n, Fr x, Fr g_scalar) {
-  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const Fr s = (g_scalar * x.pow_u64(i)).from_mont();
-  G1Affine g;
+// out[i] = [g_scalar * x^i] G1::generator, normalised to affine, by fixed-base multiplication.
+//
+// The generator never changes, so its signed-window table is built once per process (srs_gen_table):
+//   T[w][d - 1] = [d * 2^(kSetupC * w)] G,   w < kSetupW, d = 1 .. 2^(kSetupC - 1)   (32 x 128 points, 384 KiB).
+// A scalar below r < 2^255 recoded into signed 8-bit digits has kSetupW = 32 windows, the top one at most 128, so
+// [s]G is one mixed addition per non-zero digit and no doubling at all.
+static constexpr int kSetupC = 8, kSetupW = 32, kSetupHalf = 1 << (kSetupC - 1);
+
+PB_D G1Affine g1_generator() {  // G1Affine::generator(), Montgomery limbs
   const uint32_t gx[12] = {0xfd530c16u, 0x5cb38790u, 0x9976fff5u, 0x7817fc67u, 0x143ba1c1u, 0x154f95c7u,
                            0xf3d0e747u, 0xf0ae6acdu, 0x21dbf440u, 0xedce6eccu, 0x9e0bfb75u, 0x12017741u};
   const uint32_t gy[12] = {0x0ce72271u, 0xbaac93d5u, 0x7918fd8eu, 0x8c22631au, 0x570725ceu, 0xdd595f13u,
                            0x50405194u, 0x51ac5829u, 0xad0059c0u, 0x0e1c8c3fu, 0x5008a26au, 0x0bbc3efcu};
+  G1Affine g;
 #pragma unroll
   for (int k = 0; k < 12; k++) {
     g.x.v[k] = gx[k];
     g.y.v[k] = gy[k];
   }
-  G1Xyzz acc = G1Xyzz::identity();
+  return g;
+}
+
+// One thread per table entry: [d * 2^(8w)] G by double-and-add (once per process, 4096 threads).
+__global__ void __launch_bounds__(128) k_srs_gen_table(uint4* table) {
+  const int t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= kSetupW * kSetupHalf) return;
+  const int w = t / kSetupHalf, d = t % kSetupHalf + 1;
+  uint32_t k[8] = {0, 0, 0, 0, 0, 0, 0, 0};  // d * 2^(8w) < 2^255
+  const int bit = kSetupC * w;
+  k[bit / 32] = (uint32_t)d << (bit % 32);
+  if (bit % 32 > 24) k[bit / 32 + 1] = (uint32_t)d >> (32 - bit % 32);
+  st_affine(table, t, xyzz_to_affine(xyzz_mul(G1Xyzz::from_affine(g1_generator()), k, 8)));
+}
+
+// Thread t owns the run [t * run, min(n, (t + 1) * run)) of powers.  It forms g_scalar * x^i by one pow for the first
+// index and one Fr product per step, sums one table point per non-zero signed digit into an XYZZ accumulator, and
+// normalises the whole run with one inversion (Montgomery's trick): per point it keeps X * ZZZ and Y * ZZ in out[i] and
+// q = ZZ * ZZZ and the running product of the q's in `scratch` ([run][threads] pairs of Fp, so a warp's accesses are
+// contiguous); then x = X ZZZ / q and y = Y ZZ / q walking the run backwards.  g_scalar * x^i is never zero - both
+// draws are nonzero and r is prime - so no accumulator ends at the identity and every q is invertible.
+__global__ void __launch_bounds__(128) k_srs_setup(uint4* out, size_t n, Fr x, Fr g_scalar, const uint4* __restrict__ table,
+                                                   uint4* scratch, unsigned run) {
+  const size_t threads = (size_t)gridDim.x * blockDim.x, t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const size_t first = t * run;
+  if (first >= n) return;
+  const unsigned m = (unsigned)min((size_t)run, n - first);
+  Fr p = g_scalar * x.pow_u64(first);
+  Fp prod = Fp::one();
 #pragma unroll 1
-  for (int w = 7; w >= 0; w--) {
+  for (unsigned j = 0; j < m; j++) {
+    const Fr s = p.from_mont();
+    p = p * x;
+    G1Xyzz acc = G1Xyzz::identity();
+    unsigned carry = 0;
 #pragma unroll 1
-    for (int b = 31; b >= 0; b--) {
-      acc = xyzz_dbl(acc);
-      if ((s.v[w] >> b) & 1u) xyzz_madd(acc, g.x, g.y);
+    for (int w = 0; w < kSetupW; w++) {
+      int d = (int)((s.v[w / 4] >> (8 * (w % 4))) & 0xffu) + (int)carry;
+      carry = d > kSetupHalf;
+      if (carry) d -= 1 << kSetupC;
+      if (d == 0) continue;
+      const G1Affine pt = ld_affine(table, (size_t)w * kSetupHalf + (d > 0 ? d : -d) - 1);
+      xyzz_madd(acc, pt.x, d > 0 ? pt.y : pt.y.neg());
     }
+    const Fp zz = acc.zz.canonical(), zzz = acc.zzz.canonical();
+    const Fp q = zz * zzz;
+    prod = prod * q;
+    G1Affine xy;
+    xy.x = acc.x.canonical() * zzz;
+    xy.y = acc.y.canonical() * zz;
+    st_affine(out, first + j, xy);
+    uint4* sc = scratch + 6 * (j * threads + t);
+    st_fp(sc, q);
+    st_fp(sc + 3, prod);
   }
-  st_affine(out, i, xyzz_to_affine(acc));
+  Fp inv = fp_inv_bingcd(prod);  // 1 / (q_0 ... q_{m-1})
+#pragma unroll 1
+  for (unsigned j = m; j-- > 0;) {
+    const uint4* sc = scratch + 6 * (j * threads + t);
+    const Fp iq = j ? inv * ld_fp(sc - 6 * threads + 3) : inv;  // 1 / q_j
+    inv = inv * ld_fp(sc);
+    G1Affine xy;  // plain loads: out[] was written by this kernel, so not through the read-only path
+    xy.x = ld_fp(out + 6 * (first + j)) * iq;
+    xy.y = ld_fp(out + 6 * (first + j) + 3) * iq;
+    st_affine(out, first + j, xy);
+  }
 }
 
 // G1Affine::from_slice for a whole commit key (CommitKey::from_slice, reference
@@ -1630,17 +1691,48 @@ int srs_from_device(const uint4* d_points, size_t n_points, pb200_srs** out, int
   return 0;
 }
 
+// The generator's window table of k_srs_setup, built on first use and kept for the life of the process.
+static int srs_gen_table(const uint4** out) {
+  static std::once_flag once;
+  static uint4* table = nullptr;
+  static cudaError_t err = cudaSuccess;
+  std::call_once(once, [] {
+    cudaStream_t st = thread_stream();
+    err = cudaMalloc((void**)&table, (size_t)kSetupW * kSetupHalf * 96);
+    if (err == cudaSuccess) {
+      PB_LAUNCH(k_srs_gen_table, div_up(kSetupW * kSetupHalf, 128), 128, 0, st, table);
+      err = cudaGetLastError();
+    }
+    if (err == cudaSuccess) err = cudaStreamSynchronize(st);
+  });
+  if (err != cudaSuccess) return fail(PB200_ERR_CUDA, "generator table for the commit-key setup", cudaGetErrorString(err));
+  *out = table;
+  return 0;
+}
+
 int srs_setup(const uint64_t* x_mont, const uint64_t* g_scalar_mont, size_t n, uint8_t* out_raw) {
+  const uint4* table = nullptr;
+  PB_TRY(srs_gen_table(&table));
   cudaStream_t st = thread_stream();
-  uint4* d = nullptr;
+  // Runs of up to 32 points share an inversion; shorter runs keep about 1024 threads per SM busy on small keys.
+  const size_t want_threads = (size_t)std::max(1u, num_sms()) * 1024;
+  const unsigned run = (unsigned)std::min<size_t>(32, std::max<size_t>(1, div_up(n, want_threads)));
+  const size_t threads = div_up(div_up(n, run), 128) * 128;
+  uint4 *d = nullptr, *scratch = nullptr;  // plain allocations: a large key's buffers do not stay in the stream pool
   PB_CUDA(cudaMalloc((void**)&d, n * 96));
+  cudaError_t e = cudaMalloc((void**)&scratch, (size_t)run * threads * 96);
   Fr x, gs;
   memcpy(x.v, x_mont, 32);
   memcpy(gs.v, g_scalar_mont, 32);
-  PB_LAUNCH(k_srs_setup, div_up(n, 64), 64, 0, st, d, n, x, gs);
-  PB_CUDA(cudaMemcpyAsync(out_raw, d, n * 96, cudaMemcpyDeviceToHost, st));
-  PB_CUDA(cudaStreamSynchronize(st));
+  if (e == cudaSuccess) {
+    PB_LAUNCH(k_srs_setup, threads / 128, 128, 0, st, d, n, x, gs, table, scratch, run);
+    e = cudaGetLastError();
+  }
+  if (e == cudaSuccess) e = cudaMemcpyAsync(out_raw, d, n * 96, cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
   cudaFree(d);
+  cudaFree(scratch);
+  PB_CUDA(e);
   return 0;
 }
 

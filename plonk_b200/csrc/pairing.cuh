@@ -293,6 +293,47 @@ PB_NOINL bool g2_decode(const uint8_t* b, G2Affine* out) {
   return acc.z.is_zero();
 }
 
+// [k] q for a canonical little-endian scalar of 8 words (double-and-add, variable time: the setup draws are the
+// caller's, and this runs once per PublicParameters::setup).
+PB_NOINL G2Jac g2_mul(const G2Affine& q, const uint32_t* k) {
+  G2Jac acc = {Fp2::one(), Fp2::one(), Fp2::zero()};
+#pragma unroll 1
+  for (int w = 7; w >= 0; w--) {
+#pragma unroll 1
+    for (int bit = 31; bit >= 0; bit--) {
+      acc = g2_dbl(acc);
+      if ((k[w] >> bit) & 1u) acc = g2_madd(acc, q);
+    }
+  }
+  return acc;
+}
+
+PB_NOINL G2Affine g2_to_affine(const G2Jac& p) {
+  if (p.z.is_zero()) return {Fp2::zero(), Fp2::zero(), true};
+  const Fp2 zi = p.z.inv(), zi2 = zi.sqr();
+  return {p.x * zi2, p.y * zi2 * zi, false};
+}
+
+// G2Affine::to_compressed, the inverse of g2_decode: x.c1 then x.c0 big-endian, bit 7 set, bit 6 for the identity,
+// bit 5 when y is the lexicographically larger root (c1 compared first, c0 when c1 = 0).
+PB_NOINL void g2_encode(const G2Affine& q, uint8_t* b) {
+  for (int k = 0; k < 96; k++) b[k] = 0;
+  if (q.inf) {
+    b[0] = 0xc0u;
+    return;
+  }
+  const Fp xc[2] = {q.x.c1.from_mont(), q.x.c0.from_mont()};
+  for (int h = 0; h < 2; h++)
+    for (int k = 0; k < 12; k++) {
+      const int o = 48 * h + 44 - 4 * k;
+      b[o] = (uint8_t)(xc[h].v[k] >> 24);
+      b[o + 1] = (uint8_t)(xc[h].v[k] >> 16);
+      b[o + 2] = (uint8_t)(xc[h].v[k] >> 8);
+      b[o + 3] = (uint8_t)xc[h].v[k];
+    }
+  b[0] |= 0x80u | (q.y.lex_largest() ? 0x20u : 0u);
+}
+
 // ---- Miller loop --------------------------------------------------------------------------------------------
 // |x| of BLS12-381; x itself is negative
 #define PB_BLS_X 0xd201000000010000ull

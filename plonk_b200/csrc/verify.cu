@@ -321,7 +321,25 @@ __global__ void k_g2_prepare(const uint8_t* enc, int count, LineCoeffs* lines, i
   G2Affine q;
   const bool valid = g2_decode(enc + 96 * k, &q);
   ok[k] = !valid ? 0 : (q.inf ? 2 : 1);
-  if (valid && !q.inf) g2_prepare(q, lines + (size_t)PB_G2_LINES * k);
+  if (valid && !q.inf && lines) g2_prepare(q, lines + (size_t)PB_G2_LINES * k);
+}
+
+// The G2 half of PublicParameters::setup (srs.rs:91-93): h = [h_scalar] G2Affine::generator() and x_h = [x] h, written
+// as two 96-byte compressed points (h, then x_h).  Scalars in Montgomery form.  One thread: two scalar multiplications.
+__global__ void k_opening_key_g2(Fr x, Fr h_scalar, uint8_t* out) {
+  if (blockIdx.x || threadIdx.x) return;
+  const uint8_t gen[96] = {  // G2Affine::generator().to_compressed()
+      0x93, 0xe0, 0x2b, 0x60, 0x52, 0x71, 0x9f, 0x60, 0x7d, 0xac, 0xd3, 0xa0, 0x88, 0x27, 0x4f, 0x65, 0x59, 0x6b, 0xd0, 0xd0,
+      0x99, 0x20, 0xb6, 0x1a, 0xb5, 0xda, 0x61, 0xbb, 0xdc, 0x7f, 0x50, 0x49, 0x33, 0x4c, 0xf1, 0x12, 0x13, 0x94, 0x5d, 0x57,
+      0xe5, 0xac, 0x7d, 0x05, 0x5d, 0x04, 0x2b, 0x7e, 0x02, 0x4a, 0xa2, 0xb2, 0xf0, 0x8f, 0x0a, 0x91, 0x26, 0x08, 0x05, 0x27,
+      0x2d, 0xc5, 0x10, 0x51, 0xc6, 0xe4, 0x7a, 0xd4, 0xfa, 0x40, 0x3b, 0x02, 0xb4, 0x51, 0x0b, 0x64, 0x7a, 0xe3, 0xd1, 0x77,
+      0x0b, 0xac, 0x03, 0x26, 0xa8, 0x05, 0xbb, 0xef, 0xd4, 0x80, 0x56, 0xc8, 0xc1, 0x21, 0xbd, 0xb8};
+  G2Affine g;
+  g2_decode(gen, &g);
+  const Fr hs = h_scalar.from_mont(), xs = x.from_mont();
+  const G2Affine h = g2_to_affine(g2_mul(g, hs.v));
+  g2_encode(h, out);
+  g2_encode(g2_to_affine(g2_mul(h, xs.v)), out + 96);
 }
 
 // e(P_k, Q_k) as an Fp12 (tests only); an identity on either side gives 1.
@@ -368,6 +386,25 @@ int g2_prepare_dev(const uint8_t* enc, int count, LineCoeffs* d_lines, int* ok, 
   return 0;
 }
 
+// OpeningKey::from_bytes (key.rs:609-648): g, h and [x]h decoded with the on-curve and subgroup checks, the identity
+// refused (OpeningKey::try_new).  g_raw (96 bytes) receives g when given; d_lines, when given, the prepared lines of
+// [x]h then h.
+int opening_key_decode(const uint8_t* opening_key, uint8_t* g_raw, LineCoeffs* d_lines) {
+  uint8_t raw[96];
+  PB_TRY(g1_decompress(opening_key, 1, 1, raw));
+  bool g_inf = true;
+  for (int k = 0; k < 96; k++) g_inf = g_inf && raw[k] == 0;
+  uint8_t g2[2 * 96];
+  memcpy(g2, opening_key + 48 + 96, 96);  // [x]H first: the pair of -(W_z + u W_zw)
+  memcpy(g2 + 96, opening_key + 48, 96);
+  int ok[2] = {0, 0};
+  PB_TRY(g2_prepare_dev(g2, 2, d_lines, ok, thread_stream()));
+  if (g_inf || ok[0] != 1 || ok[1] != 1)
+    return fail(PB200_ERR_POINT_MALFORMED, "InvalidData: opening key point is the identity, not on the curve or not in the subgroup");
+  if (g_raw) memcpy(g_raw, raw, 96);
+  return 0;
+}
+
 uint64_t be64(const uint8_t* b) {
   uint64_t x = 0;
   for (int k = 0; k < 8; k++) x = (x << 8) | b[k];
@@ -385,23 +422,12 @@ constexpr size_t kVerifierKeyBytes = 20 * 48 + 8;
 int verifier_build(const uint8_t* label, size_t label_len, uint64_t vk_n, uint64_t size, uint64_t constraints, const uint8_t* comms,
                    const uint8_t* opening_key, const uint64_t* pi_idx, size_t n_pi, pb200_verifier** out) {
   PB_TRY(ensure_init());
-  // the 15 commitments and opening_key.g: checked decoding (Commitment / G1Affine::from_bytes)
-  std::vector<uint8_t> enc(16 * 48), raw(16 * 96);
-  memcpy(enc.data(), comms, 15 * 48);
-  memcpy(enc.data() + 15 * 48, opening_key, 48);
-  PB_TRY(g1_decompress(enc.data(), 16, 1, raw.data()));
-  bool g_inf = true;
-  for (int k = 0; k < 96; k++) g_inf = g_inf && raw[15 * 96 + k] == 0;
-  cudaStream_t st = thread_stream();
+  // the 15 commitments: checked decoding (Commitment / G1Affine::from_bytes); then the opening key, with its lines
+  std::vector<uint8_t> raw(16 * 96);
+  PB_TRY(g1_decompress(comms, 15, 1, raw.data()));
   LineCoeffs* d_lines = nullptr;
   PB_CUDA(cudaMalloc((void**)&d_lines, 2 * PB_G2_LINES * sizeof(LineCoeffs)));
-  uint8_t g2[2 * 96];
-  memcpy(g2, opening_key + 48 + 96, 96);  // [x]H first: the pair of -(W_z + u W_zw)
-  memcpy(g2 + 96, opening_key + 48, 96);
-  int ok[2] = {0, 0};
-  int rc = g2_prepare_dev(g2, 2, d_lines, ok, st);
-  if (rc == 0 && (g_inf || ok[0] != 1 || ok[1] != 1))
-    rc = fail(PB200_ERR_POINT_MALFORMED, "InvalidData: opening key point is the identity, not on the curve or not in the subgroup");
+  int rc = opening_key_decode(opening_key, raw.data() + 15 * 96, d_lines);
   // EvaluationDomain::new (domain.rs:118-160)
   int log_n = 0;
   while (rc == 0 && log_n < 64 && ((uint64_t)1 << log_n) < vk_n) log_n++;
@@ -612,6 +638,25 @@ int batch_verify(const pb200_verifier_t* const* Vs, const int32_t* versions, con
 }
 
 }  // namespace
+
+int opening_key_check(const uint8_t* opening_key) { return opening_key_decode(opening_key, nullptr, nullptr); }
+
+int opening_key_g2(const uint64_t* x_mont, const uint64_t* h_scalar_mont, uint8_t* out_2x96) {
+  cudaStream_t st = thread_stream();
+  Fr x, hs;
+  memcpy(x.v, x_mont, 32);
+  memcpy(hs.v, h_scalar_mont, 32);
+  uint8_t* d_out = nullptr;
+  PB_CUDA(cudaMallocAsync((void**)&d_out, 2 * 96, st));
+  PB_LAUNCH(k_opening_key_g2, 1, 32, 0, st, x, hs, d_out);
+  cudaError_t e = cudaGetLastError();
+  if (e == cudaSuccess) e = cudaMemcpyAsync(out_2x96, d_out, 2 * 96, cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  cudaFreeAsync(d_out, st);
+  PB_CUDA(e);
+  return 0;
+}
+
 }  // namespace pb
 
 using namespace pb;

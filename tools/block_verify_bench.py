@@ -15,6 +15,7 @@ import os
 import sys
 import time
 from concurrent.futures import ThreadPoolExecutor
+from types import SimpleNamespace
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -29,8 +30,6 @@ def main():
     ap.add_argument("--reps", type=int, default=5)
     a = ap.parse_args()
 
-    import ctypes
-
     import torch
 
     import plonk_b200
@@ -38,11 +37,9 @@ def main():
     from oracle import pyref as R
     from plonk_b200 import gadgets
     from plonk_b200._lib import check, lib
-    from tests.models import pairing_model as M
 
     check(lib().pb200_init(0))
-    x, gs, hs = 0x1234567, 0x7654321, 0xABCDEF
-    okey = M.opening_key_from_secret(x, gs, hs)
+    draws = [R.fr_to_mont_bytes(v) for v in (0x1234567, 0x7654321, 0xABCDEF)]  # one SRS: every circuit shares its opening key
     arrays = [(b"dusk-network", gadgets.bench_circuit(1 << log_n).arrays()) for log_n in (16, 15, 14, 13)]
     for seed in range(4):
         comp = R.Composer.initialized()
@@ -52,10 +49,8 @@ def main():
     circuits = []
     for label, arr in arrays[:max_k]:
         n = 1 << (arr.constraints + 6 - 1).bit_length()
-        srs = ctypes.create_string_buffer(96 * (n + 7))
-        check(lib().pb200_srs_setup_from_secret(R.fr_to_mont_bytes(x), R.fr_to_mont_bytes(gs), n + 7, srs))
-        prover = plonk_b200.Prover(label, arr.constraints, arr.selectors, arr.wires, arr.n_witnesses, srs.raw)
-        verifier = plonk_b200.Verifier(label, arr.constraints, prover.commitments(), okey, arr.pi_idx)
+        pp = plonk_b200.PublicParameters.setup(n, draws)
+        prover, verifier = plonk_b200.Compiler.compile(pp, label, SimpleNamespace(arrays=lambda arr=arr: arr))
         proofs = [prover.prove(arr.witnesses, arr.pi_idx, arr.pi_vals, cref.draw_blinders(R.StdRng.seed_from_u64(s))) for s in range(64)]
         del prover
         circuits.append((verifier, proofs, arr.pi_vals, arr.constraints))

@@ -34,8 +34,6 @@ def main():
     ap.add_argument("--reps", type=int, default=5)
     a = ap.parse_args()
 
-    import ctypes
-
     import torch
 
     import plonk_b200
@@ -43,16 +41,13 @@ def main():
     from oracle import cref
     from plonk_b200 import gadgets
     from plonk_b200._lib import check, lib
-    from tests.models import pairing_model as M
 
     check(lib().pb200_init(0))
-    arr = gadgets.bench_circuit(1 << a.log_n).arrays()
+    comp = gadgets.bench_circuit(1 << a.log_n)
+    arr = comp.arrays()
     n = 1 << (arr.constraints + 6 - 1).bit_length()
-    x, gs, hs = 0x1234567, 0x7654321, 0xABCDEF
-    srs = ctypes.create_string_buffer(96 * (n + 7))
-    check(lib().pb200_srs_setup_from_secret(R.fr_to_mont_bytes(x), R.fr_to_mont_bytes(gs), n + 7, srs))
-    prover = plonk_b200.Prover(b"dusk-network", arr.constraints, arr.selectors, arr.wires, arr.n_witnesses, srs.raw)
-    verifier = plonk_b200.Verifier(b"dusk-network", arr.constraints, prover.commitments(), M.opening_key_from_secret(x, gs, hs), arr.pi_idx)
+    pp = plonk_b200.PublicParameters.setup(n, [R.fr_to_mont_bytes(v) for v in (0x1234567, 0x7654321, 0xABCDEF)])
+    prover, verifier = plonk_b200.Compiler.compile(pp, b"dusk-network", comp)
     proofs = [prover.prove(arr.witnesses, arr.pi_idx, arr.pi_vals, cref.draw_blinders(R.StdRng.seed_from_u64(s))) for s in range(64)]
     pis = [arr.pi_vals] * 64
     assert verifier.verify_batch(proofs, pis) == [0] * 64, "a valid proof was rejected"
