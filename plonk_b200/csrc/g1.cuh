@@ -99,28 +99,26 @@ PB_HD G1Xyzz xyzz_dbl(const G1Xyzz& p) {
   return r;
 }
 
-// acc += (x2, +-y2) for an affine, non-identity point (madd-2008-s), all special cases handled:
-// acc = identity, acc == P (doubling), acc == -P (result is the identity).
-PB_HD void xyzz_madd(G1Xyzz& acc, const Fp& x2c, const Fp& y2c) {
-  const FpR x2 = FpR::from(x2c), y2 = FpR::from(y2c);
-  if (acc.is_inf()) {
-    acc.x = x2;
-    acc.y = y2;
-    acc.zz = FpR::one();
-    acc.zzz = FpR::one();
-    return;
-  }
-  FpR u2 = x2 * acc.zz;
-  FpR s2 = y2 * acc.zzz;
+// y or -y (as 2p - y) for a canonical y != 0: the sign of a signed-digit entry, without a borrow test
+PB_HD FpR signed_y(const Fp& y, bool neg) {
+  FpR n;
+  n.v[0] = sub_cc(FpR::MOD2(0), y.v[0]);
+#pragma unroll
+  for (int i = 1; i < FpR::N - 1; i++) n.v[i] = subc_cc(FpR::MOD2(i), y.v[i]);
+  n.v[FpR::N - 1] = subc(FpR::MOD2(FpR::N - 1), y.v[FpR::N - 1]);
+#pragma unroll
+  for (int i = 0; i < FpR::N; i++) n.v[i] = neg ? n.v[i] : y.v[i];
+  return n;
+}
+
+// The common case of madd-2008-s, given u2 = x2 * acc.zz and s2 = y2 * acc.zzz: acc += (x2, y2) when
+// u2 != acc.x, i.e. acc is neither P, -P nor the identity (whose limbs are all zero, so u2 = acc.x = 0).
+// Returns false and leaves acc as it was otherwise.  Split from the two products so that a caller can
+// reuse the registers of (x2, y2) once they are read.
+PB_HD bool xyzz_madd_distinct(G1Xyzz& acc, const FpR& u2, const FpR& s2) {
   FpR p = u2 - acc.x;
+  if (p.is_zero_mod_p()) return false;
   FpR r = s2 - acc.y;
-  if (p.is_zero_mod_p()) {
-    if (r.is_zero_mod_p())
-      acc = xyzz_dbl_affine(x2, y2);
-    else
-      acc = G1Xyzz::identity();
-    return;
-  }
   FpR pp = p.sqr();
   FpR ppp = p * pp;
   FpR q = acc.x * pp;
@@ -130,7 +128,27 @@ PB_HD void xyzz_madd(G1Xyzz& acc, const Fp& x2c, const Fp& y2c) {
   acc.y = y3;
   acc.zz = acc.zz * pp;
   acc.zzz = acc.zzz * ppp;
+  return true;
 }
+
+// acc += (x2, y2) for an affine, non-identity point (madd-2008-s), all special cases handled:
+// acc = identity, acc == P (doubling), acc == -P (result is the identity).
+PB_HD void xyzz_madd(G1Xyzz& acc, const FpR& x2, const FpR& y2) {
+  if (acc.is_inf()) {
+    acc.x = x2;
+    acc.y = y2;
+    acc.zz = FpR::one();
+    acc.zzz = FpR::one();
+    return;
+  }
+  const FpR s2 = y2 * acc.zzz;
+  if (xyzz_madd_distinct(acc, x2 * acc.zz, s2)) return;
+  if ((s2 - acc.y).is_zero_mod_p())
+    acc = xyzz_dbl_affine(x2, y2);
+  else
+    acc = G1Xyzz::identity();
+}
+PB_HD void xyzz_madd(G1Xyzz& acc, const Fp& x2, const Fp& y2) { xyzz_madd(acc, FpR::from(x2), FpR::from(y2)); }
 
 // acc += o, both XYZZ (add-2008-s), all special cases handled.
 PB_HD void xyzz_add(G1Xyzz& acc, const G1Xyzz& o) {

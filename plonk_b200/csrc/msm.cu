@@ -36,6 +36,7 @@ struct pb200_srs {
   int c;  // window width in bits
   int W;  // number of windows
   uint4* table;  // [W][n_points] affine, 96 bytes each
+  bool has_inf;  // some entry of the table is the identity (k_msm_digits then leaves such entries out)
 };
 
 namespace pb {
@@ -99,19 +100,22 @@ PB_D G1Xyzz ld_xyzz(const uint4* p, size_t i) {
   return a;
 }
 
-// table[w][i] = 2^(c*w) * table[0][i]
-__global__ void k_msm_precompute(uint4* table, size_t n, int c, int W) {
+// table[w][i] = 2^(c*w) * table[0][i]; *n_inf counts the points that are the identity in some window
+__global__ void k_msm_precompute(uint4* table, size_t n, int c, int W, unsigned* n_inf) {
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   G1Affine p = ld_affine(table, i);
+  bool inf = p.is_inf();
   for (int w = 1; w < W; w++) {
     if (!p.is_inf()) {
       G1Xyzz q = G1Xyzz::from_affine(p);
       for (int k = 0; k < c; k++) q = xyzz_dbl(q);
       p = xyzz_to_affine(q);
     }
+    inf |= p.is_inf();
     st_affine(table, (size_t)w * n + i, p);
   }
+  if (inf) atomicAdd(n_inf, 1u);
 }
 
 // PublicParameters::setup restated for the device (reference src/commitment_scheme/kzg10/srs.rs:61-100):
@@ -345,9 +349,12 @@ __global__ void __launch_bounds__(128) k_g1_compress(const uint4* __restrict__ p
   o[2] = make_uint4(be[8], be[9], be[10], be[11]);
 }
 
-// Signed-digit recoding + bucket histogram.  ebkt/epos are [batch][W][n].
+// Signed-digit recoding + bucket histogram.  ebkt/epos are [batch][W][n].  inf_table is the key's table
+// when it holds the identity (else null): a digit whose table entry is the identity adds nothing and
+// gets no entry, so that the bucket walk never meets the identity.
 __global__ void k_msm_digits(const uint4* scalars, size_t n, size_t stride, int c, int W, unsigned nb,
-                             unsigned* counts, unsigned* ebkt, unsigned* epos) {
+                             const uint4* inf_table, size_t n_table, size_t first, unsigned* counts, unsigned* ebkt,
+                             unsigned* epos) {
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const unsigned b = blockIdx.y;
@@ -378,6 +385,7 @@ __global__ void k_msm_digits(const uint4* scalars, size_t n, size_t stride, int 
       carry = 0;
     }
     const size_t slot = ((size_t)b * W + w) * n + i;
+    if (d != 0 && inf_table && ld_affine(inf_table, (size_t)w * n_table + first + i).is_inf()) d = 0;
     if (d == 0) {
       ebkt[slot] = 0xffffffffu;
     } else {
@@ -510,6 +518,45 @@ PB_D G1Xyzz shfl_down_xyzz(const G1Xyzz& p, int delta, int width) {
   return r;
 }
 
+// The rare step of a bucket walk, out of line so that its doubling stays off the walk's code path: acc is
+// P, -P or the identity (after an earlier P + (-P)) for the entry e.
+__device__ __noinline__ G1Xyzz bucket_step_cold(G1Xyzz acc, const uint4* table, unsigned e) {
+  const G1Affine pt = ld_affine(table, e >> 1);
+  xyzz_madd(acc, FpR::from(pt.x), signed_y(pt.y, e & 1u));
+  return acc;
+}
+
+// The sum of the entries src[k], src[k + step], ... below hi (the identity when there is none).  An entry is
+// (table index << 1 | sign); the table holds no identity (k_msm_digits leaves those entries out).  The first
+// entry starts the sum, and the next entry's load is issued as soon as the current point has gone into its
+// two products, into the same registers, so it is in flight during the rest of the addition.
+PB_D G1Xyzz bucket_walk(const uint4* table, const unsigned* src, unsigned k, unsigned hi, unsigned step) {
+  if (k >= hi) return G1Xyzz::identity();
+  unsigned e = __ldg(src + k);
+  G1Affine pt = ld_affine(table, e >> 1);
+  G1Xyzz acc;
+  acc.x = FpR::from(pt.x);
+  acc.y = signed_y(pt.y, e & 1u);
+  acc.zz = FpR::one();
+  acc.zzz = FpR::one();
+  k += step;
+  if (k < hi) {
+    e = __ldg(src + k);
+    pt = ld_affine(table, e >> 1);
+  }
+  for (; k < hi; k += step) {
+    const FpR u2 = FpR::from(pt.x) * acc.zz;
+    const FpR s2 = signed_y(pt.y, e & 1u) * acc.zzz;
+    const unsigned cur = e;
+    if (k + step < hi) {
+      e = __ldg(src + k + step);
+      pt = ld_affine(table, e >> 1);
+    }
+    if (!xyzz_madd_distinct(acc, u2, s2)) acc = bucket_step_cold(acc, table, cur);
+  }
+  return acc;
+}
+
 // Bucket accumulation: thread = (bucket, part); the 2^log_split parts of a bucket are adjacent
 // lanes and are merged with a warp-shuffle tree, so `sums` holds one XYZZ point per bucket
 // ([batch][nb]).  Buckets are visited in `order` (largest first, near-equal sizes per warp).
@@ -533,38 +580,22 @@ __global__ void __launch_bounds__(THREADS, MIN_CTAS) k_msm_accumulate(const uint
     lo = min(end, start + part * chunk);
     hi = min(end, lo + chunk);
   }
-  const unsigned* src = sorted + (size_t)b * cap;
-  G1Xyzz acc = G1Xyzz::identity();
-  // software pipeline: the (random, 96-byte) load of the next point is in flight during the ~3000
-  // integer instructions of the current addition
-  unsigned e_next = 0;
-  G1Affine p_next;
-  if (lo < hi) {
-    e_next = __ldg(src + lo);
-    p_next = ld_affine(table, e_next >> 1);
-  }
-  for (unsigned k = lo; k < hi; k++) {
-    const unsigned e = e_next;
-    G1Affine p = p_next;
-    if (k + 1 < hi) {
-      e_next = __ldg(src + k + 1);
-      p_next = ld_affine(table, e_next >> 1);
-    }
-    if (p.is_inf()) continue;
-    if (e & 1u) p.y = p.y.neg();
-    xyzz_madd(acc, p.x, p.y);
-  }
+  G1Xyzz acc = bucket_walk(table, sorted + (size_t)b * cap, lo, hi, 1);
   for (int d = (int)split >> 1; d > 0; d >>= 1) {
     G1Xyzz o = shfl_down_xyzz(acc, d, (int)split);
-    xyzz_add(acc, o);
+    if (part + d < split) xyzz_add(acc, o);
   }
   if (valid && part == 0) st_xyzz(sums, (size_t)b * nb + bucket, acc);
 }
 
+// The sum lands in lane 0.  A lane whose partner is past the end of the warp gets its own value back from the
+// shuffle; it skips the addition (a doubling, which would serialise with the other lanes' additions) because
+// lane 0 never reads what it holds.
 PB_D G1Xyzz warp_sum(G1Xyzz v) {
+  const unsigned lane = threadIdx.x & 31;
   for (int d = 16; d > 0; d >>= 1) {
     G1Xyzz o = shfl_down_xyzz(v, d, 32);
-    xyzz_add(v, o);
+    if (lane + d < 32) xyzz_add(v, o);
   }
   return v;
 }
@@ -595,15 +626,7 @@ __global__ void __launch_bounds__(128) k_msm_heavy_chunks(const uint4* table, co
     }
     const unsigned bucket = ord[lo];
     const unsigned start = off[bucket] + (v - hp[lo]) * heavy_chunk, end = min(off[bucket + 1], start + heavy_chunk);
-    G1Xyzz acc = G1Xyzz::identity();
-    for (unsigned k = start + lane; k < end; k += 32) {
-      const unsigned e = __ldg(src + k);
-      G1Affine p = ld_affine(table, e >> 1);
-      if (p.is_inf()) continue;
-      if (e & 1u) p.y = p.y.neg();
-      xyzz_madd(acc, p.x, p.y);
-    }
-    acc = warp_sum(acc);
+    G1Xyzz acc = warp_sum(bucket_walk(table, src, start + lane, end, 32));
     if (lane == 0) st_xyzz(partials, (size_t)b * part_cap + v, acc);
   }
 }
@@ -1075,7 +1098,7 @@ PB_D G1Xyzz weighted_lane_sum(G1Xyzz x, int lane, int n, int first) {
   G1Xyzz y = (lane >= first && lane < n) ? x : G1Xyzz::identity();
   for (int d = n >> 1; d > 0; d >>= 1) {
     G1Xyzz o = shfl_down_xyzz(y, d, 32);
-    xyzz_add(y, o);
+    if (lane + d < n) xyzz_add(y, o);
   }
   return y;
 }
@@ -1356,7 +1379,7 @@ static int msm_enqueue(const pb200_srs* srs, size_t first, const uint64_t* d_sca
   PB_CUDA(cudaMemsetAsync(counts, 0, s.bytes[kCounts], st));
 
   PB_LAUNCH(k_msm_digits, dim3(div_up(n, 128), batch), 128, 0, st, (const uint4*)d_scalars, n, stride, c, W, nb,
-            counts, ebkt, epos);
+            srs->has_inf ? (const uint4*)srs->table : nullptr, srs->n_points, first, counts, ebkt, epos);
   int size_shift = 0;  // size unit: average bucket ~ 64 units
   while (((cap / nb) >> size_shift) > 64) size_shift++;
   const unsigned heavy_chunk = shape.wide_heavy_chunks ? kHeavyChunkWide : kHeavyChunk;
@@ -1633,6 +1656,23 @@ size_t msm_workspace_bytes(const pb200_srs* srs, size_t n, uint32_t batch) {
   return total;
 }
 
+// The windows w >= 1 of a table whose window 0 is on the device, and whether any entry is the identity.
+static cudaError_t srs_fill_windows(pb200_srs* s, cudaStream_t st) {
+  unsigned* d_inf = nullptr;
+  unsigned n_inf = 0;
+  cudaError_t e = cudaMalloc((void**)&d_inf, sizeof(unsigned));
+  if (e == cudaSuccess) e = cudaMemsetAsync(d_inf, 0, sizeof(unsigned), st);
+  if (e == cudaSuccess) {
+    PB_LAUNCH(k_msm_precompute, div_up(s->n_points, 64), 64, 0, st, s->table, s->n_points, s->c, s->W, d_inf);
+    e = cudaGetLastError();
+  }
+  if (e == cudaSuccess) e = cudaMemcpyAsync(&n_inf, d_inf, sizeof(unsigned), cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  cudaFree(d_inf);
+  s->has_inf = n_inf != 0;
+  return e;
+}
+
 int srs_upload(const uint8_t* raw, size_t n_points, pb200_srs** out, int window_bits) {
   if (n_points == 0) return fail(PB200_ERR_INVALID_ARG, "empty commit key");
   cudaStream_t st = thread_stream();
@@ -1647,10 +1687,7 @@ int srs_upload(const uint8_t* raw, size_t n_points, pb200_srs** out, int window_
     return fail(PB200_ERR_CUDA, "cudaMalloc(commit key table)", cudaGetErrorString(e));
   }
   e = cudaMemcpyAsync(s->table, raw, n_points * 96, cudaMemcpyHostToDevice, st);
-  if (e == cudaSuccess) {
-    PB_LAUNCH(k_msm_precompute, div_up(n_points, 64), 64, 0, st, s->table, n_points, s->c, s->W);
-    e = cudaStreamSynchronize(st);
-  }
+  if (e == cudaSuccess) e = srs_fill_windows(s, st);
   if (e != cudaSuccess) {
     cudaFree(s->table);
     delete s;
@@ -1678,10 +1715,7 @@ int srs_from_device(const uint4* d_points, size_t n_points, pb200_srs** out, int
     return fail(PB200_ERR_CUDA, "cudaMalloc(commit key table)", cudaGetErrorString(e));
   }
   e = cudaMemcpyAsync(s->table, d_points, n_points * 96, cudaMemcpyDeviceToDevice, st);
-  if (e == cudaSuccess) {
-    PB_LAUNCH(k_msm_precompute, div_up(n_points, 64), 64, 0, st, s->table, n_points, s->c, s->W);
-    e = cudaStreamSynchronize(st);
-  }
+  if (e == cudaSuccess) e = srs_fill_windows(s, st);
   if (e != cudaSuccess) {
     cudaFree(s->table);
     delete s;
