@@ -14,6 +14,7 @@ for f in capi ntt msm prover ecntt verify; do
 done
 g++ -std=c++17 -O2 -fPIC -c -o $OBJ/host_field.o $SRC/host_field.cpp
 g++ -std=c++17 -O2 -fPIC -c -o $OBJ/composer.o $SRC/composer.cpp
+g++ -std=c++17 -O2 -fPIC -c -o $OBJ/compress.o $SRC/compress.cpp
 for p in "${pids[@]}"; do wait $p; done
-nvcc -shared -o "$OUT" $OBJ/capi.o $OBJ/ntt.o $OBJ/msm.o $OBJ/prover.o $OBJ/ecntt.o $OBJ/verify.o $OBJ/host_field.o $OBJ/composer.o
+nvcc -shared -o "$OUT" $OBJ/capi.o $OBJ/ntt.o $OBJ/msm.o $OBJ/prover.o $OBJ/ecntt.o $OBJ/verify.o $OBJ/host_field.o $OBJ/composer.o $OBJ/compress.o
 echo "built $OUT"

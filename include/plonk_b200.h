@@ -28,6 +28,10 @@
  *   pb200_batch_verify_groups        the same over groups under several verifiers and versions (one SRS)
  *   pb200_public_parameters_setup    PublicParameters::setup      src/commitment_scheme/kzg10/srs.rs:61-100
  *   pb200_opening_key_check          OpeningKey::from_bytes       src/commitment_scheme/kzg10/key.rs:609-648
+ *   pb200_circuit_compress           Circuit::compress / CompressedCircuit::from_composer
+ *                                    src/composer/circuit.rs:28-45, src/composer/compress.rs:136-240
+ *   pb200_compressed_circuit_info / pb200_prover_from_compressed
+ *                                    Compiler::compile_with_compressed   src/compiler.rs:84-112, compress.rs:242-461
  *   (Compiler::compile, src/compiler.rs:116-461, is pb200_prover_new, pb200_prover_commitments and pb200_verifier_new
  *    in sequence; the mirrors write it once.)
  *
@@ -67,7 +71,10 @@ typedef enum {
                                      not canonical, not on the curve or not in the prime-order subgroup */
   PB200_ERR_VERIFY = -11,         /* Error::ProofVerificationError: the proof does not satisfy the verifier */
   PB200_ERR_UNSUPPORTED_VERSION = -12,/* Error::UnsupportedProvingVersion: PlonkVersion::V1 proofs cannot be made */
-  PB200_ERR_DEGREE_IS_ZERO = -13  /* Error::DegreeIsZero: PublicParameters::setup with max_degree = 0 (srs.rs:65-68) */
+  PB200_ERR_DEGREE_IS_ZERO = -13, /* Error::DegreeIsZero: PublicParameters::setup with max_degree = 0 (srs.rs:65-68) */
+  PB200_ERR_INVALID_COMPRESSED = -14,/* Error::InvalidCompressedCircuit: a compressed circuit that does not inflate, unpack or
+                                        validate within the public parameters' bounds (compress.rs:242-334) */
+  PB200_ERR_SCALAR_MALFORMED = -15 /* Error::BlsScalarMalformed: a compressed circuit's scalar is not canonical (compress.rs:329-335) */
 } pb200_status;
 
 /* PlonkVersion (src/compiler.rs:22-42), for the *_with_version calls.  V3 is the current profile and the one the
@@ -286,6 +293,37 @@ int pb200_prove_with_version(const pb200_prover_t* prover, int version, const ui
 int pb200_prove_dev_with_version(const pb200_prover_t* prover, int version, const uint64_t* d_witnesses, size_t n_witnesses,
                                  const uint64_t* pi_idx, const uint64_t* pi_vals, size_t n_pi,
                                  const uint64_t* blinders, uint8_t* out_proof, void* stream);
+
+/* ---- compressed circuits (Circuit::compress, Compiler::compile_with_compressed) ----------------------------------- */
+/* CompressedCircuit::from_composer (src/composer/compress.rs:136-240; Circuit::compress, circuit.rs:28-45): the circuit
+ * as pb200_prover_new takes it (selectors in Montgomery form, wires, the witness count) plus its public-input positions,
+ * as MessagePack (layout: DESIGN.md section 2) behind raw deflate at level 9.  hades_optimization != 0 seeds the scalar
+ * table with the Hades round constants and MDS entries, as Circuit::compress always does.  The inflated payload is the
+ * reference's packing; the deflate bytes are zlib's, not miniz_oxide's.  Host only, no device needed.  *len always
+ * receives the size; out = NULL writes nothing else; cap < *len is PB200_ERR_INVALID_ARG and `out` is left untouched.
+ * A wire index >= n_witnesses or a repeated / out-of-range public-input position is PB200_ERR_INVALID_ARG.  zlib
+ * (libz.so.1) is loaded at run time; without it the call is PB200_ERR_NOT_READY. */
+int pb200_circuit_compress(size_t n_constraints, const uint64_t* selectors, const uint32_t* wires, size_t n_witnesses,
+                           const uint64_t* pi_idx, size_t n_pi, int hades_optimization,
+                           uint8_t* out, size_t cap, size_t* len);
+/* CompressedCircuit::from_bytes (compress.rs:303-450) with the bounds Compiler::compile_with_compressed derives from
+ * public parameters of n_srs_points points (compiler.rs:84-112), without building anything.  In the reference's order:
+ * the packed-size limit max_constraints x 857 + 30, inflation within it, unpacking with every array bounded and no
+ * trailing bytes, index validation (all PB200_ERR_INVALID_COMPRESSED), then the canonical check of every serialized
+ * scalar (PB200_ERR_SCALAR_MALFORMED).  Any raw-deflate stream is accepted.  Returns the gate count, the circuit's
+ * witness count, n_labels (the distinct witness labels the gates use: the witnesses of the reference's rebuilt
+ * composer) and the public-input count; pi_idx != NULL also receives the *n_pi positions.  Host only.  zlib as above. */
+int pb200_compressed_circuit_info(const uint8_t* bytes, size_t len, size_t n_srs_points, size_t* n_constraints,
+                                  uint64_t* n_witnesses, size_t* n_labels, size_t* n_pi, uint64_t* pi_idx);
+/* Compiler::compile_with_compressed's Prover half: pb200_compressed_circuit_info's decoding, then Prover::new for the
+ * described circuit.  Only the scalar table, the P x 11 polynomial table and one polynomial index per gate go to the
+ * device, where the 11 selector columns are expanded; witness labels are renumbered densely (remap_witness,
+ * compress.rs:289-301) so that host work and memory follow the gate count, never the claimed witness count.  The
+ * prover keeps the circuit's own numbering: pb200_prove* take the witness table of the re-run circuit (the described
+ * witness count), as for a prover from pb200_prover_new, and pb200_prover_to_bytes writes what the directly compiled
+ * prover writes.  A description without gates is PB200_ERR_INVALID_ARG ("empty circuit"), as for pb200_prover_new. */
+int pb200_prover_from_compressed(const uint8_t* label, size_t label_len, const uint8_t* bytes, size_t len,
+                                 const uint8_t* srs_raw, size_t n_srs_points, pb200_prover_t** out);
 
 /* ---- verifier (Verifier::verify and verify_with_version; src/compiler/verifier.rs) ----------------------------- */
 /* Compiler::compile's Verifier half: the label, the circuit's constraint count, the 15 verifier-key commitments in

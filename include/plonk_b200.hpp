@@ -14,7 +14,9 @@
 //   plonk_b200::PlonkVersion       src/compiler.rs:22-42
 //   plonk_b200::PublicParameters   src/commitment_scheme/kzg10/srs.rs:61-196           setup, from_slice, from_slice_unchecked,
 //                                                                                      to_var_bytes, to_raw_var_bytes, max_degree
-//   plonk_b200::Compiler           src/compiler.rs:47-113, 116-461                     compile, compile_with_circuit
+//   plonk_b200::Compiler           src/compiler.rs:47-113, 116-461                     compile, compile_with_circuit,
+//                                                                                      compile_with_compressed
+//   plonk_b200::compress           src/composer/circuit.rs:28-45, src/composer/compress.rs:136-240   Circuit::compress
 //   plonk_b200::Composer           src/composer.rs:72-495 + src/composer/{bits,range,logic,truncate,select,
 //                                  point,fixed_base}.rs (host-side circuit front end, plonk_b200_composer.h)
 //   plonk_b200::Error              src/error.rs:21-120 (the variants this path can produce)
@@ -48,7 +50,9 @@ struct Error : std::runtime_error {
     UnsupportedProvingVersion, // Error::UnsupportedProvingVersion
     DegreeIsZero,              // Error::DegreeIsZero: PublicParameters::setup with max_degree = 0
     TruncatedDegreeTooLarge,   // Error::TruncatedDegreeTooLarge: Compiler::compile with too small public parameters
-    NotEnoughBytes             // Error::NotEnoughBytes: PublicParameters::from_slice of at most OpeningKey::SIZE bytes
+    NotEnoughBytes,            // Error::NotEnoughBytes: PublicParameters::from_slice of at most OpeningKey::SIZE bytes
+    InvalidCompressedCircuit,  // Error::InvalidCompressedCircuit: Compiler::compile_with_compressed refuses the description
+    BlsScalarMalformed         // Error::BlsScalarMalformed: a compressed circuit's scalar is not canonical
   };
   Kind kind;
   Error(Kind k, const std::string& what) : std::runtime_error(what), kind(k) {}
@@ -67,6 +71,8 @@ inline void check(int rc) {
     case PB200_ERR_JUBJUB_SCALAR: throw Error(Error::JubJubScalarMalformed, msg);
     case PB200_ERR_UNSUPPORTED_VERSION: throw Error(Error::UnsupportedProvingVersion, msg);
     case PB200_ERR_DEGREE_IS_ZERO: throw Error(Error::DegreeIsZero, msg);
+    case PB200_ERR_INVALID_COMPRESSED: throw Error(Error::InvalidCompressedCircuit, msg);
+    case PB200_ERR_SCALAR_MALFORMED: throw Error(Error::BlsScalarMalformed, msg);
     default: throw Error(Error::BackendFailure, msg);
   }
 }
@@ -376,6 +382,16 @@ class Prover {
     check(pb200_prover_from_bytes(bytes, len, wires.data(), n_witnesses, &p->h_));
     return p;
   }
+  // Compiler::compile_with_compressed's Prover (compiler.rs:84-112): the selector columns are expanded on the device;
+  // prove takes the re-run circuit's witness table (n_witnesses entries, the description's count)
+  static std::unique_ptr<Prover> from_compressed(const std::string& label, const std::vector<uint8_t>& compressed, const uint8_t* srs_raw,
+                                                 size_t n_srs_points, size_t n_witnesses) {
+    std::unique_ptr<Prover> p(new Prover());
+    p->n_witnesses_ = n_witnesses;
+    check(pb200_prover_from_compressed((const uint8_t*)label.data(), label.size(), compressed.data(), compressed.size(), srs_raw,
+                                       n_srs_points, &p->h_));
+    return p;
+  }
   // Prover::serialized_size (prover.rs:233-235) and Prover::to_bytes (:238-263): the bytes try_from_bytes reads
   size_t serialized_size() const {
     size_t n = 0;
@@ -657,6 +673,42 @@ struct Compiler {
     circuit(composer);
     return compile(pp, label, composer);
   }
+  // Compiler::compile_with_compressed (compiler.rs:84-112) for the bytes of compress(): the public parameters bound
+  // the decoding.  Throws InvalidCompressedCircuit or BlsScalarMalformed for a description they refuse.
+  static Pair compile_with_compressed(const PublicParameters& pp, const std::string& label, const std::vector<uint8_t>& compressed) {
+    size_t n_constraints = 0, n_labels = 0, n_pi = 0;
+    uint64_t n_witnesses = 0;
+    check(pb200_compressed_circuit_info(compressed.data(), compressed.size(), pp.points(), &n_constraints, &n_witnesses, &n_labels,
+                                        &n_pi, nullptr));
+    std::vector<uint64_t> pi_idx(n_pi);
+    if (n_pi)
+      check(pb200_compressed_circuit_info(compressed.data(), compressed.size(), pp.points(), &n_constraints, &n_witnesses, &n_labels,
+                                          &n_pi, pi_idx.data()));
+    Pair out;
+    out.first = Prover::from_compressed(label, compressed, pp.raw_points().data(), pp.points(), (size_t)n_witnesses);
+    std::array<uint8_t, 15 * 48> comms;
+    check(pb200_prover_commitments(out.first->handle(), comms.data()));
+    out.second.reset(new Verifier(label, n_constraints, comms, pp.opening_key(), pi_idx));
+    return out;
+  }
 };
+
+// Circuit::compress (circuit.rs:28-45, CompressedCircuit::from_composer compress.rs:136-240): circuit(composer) fills a
+// fresh Composer::initialized(), whose description is returned as MessagePack behind raw deflate.  The reference always
+// sets hades_optimization.
+template <class F>
+std::vector<uint8_t> compress(F&& circuit, bool hades_optimization = true) {
+  Composer composer;
+  circuit(composer);
+  const Composer::Export e = composer.finish();
+  size_t n = 0;
+  const int hades = hades_optimization ? 1 : 0;
+  check(pb200_circuit_compress(e.n_constraints, e.selectors.empty() ? nullptr : e.selectors[0].data(), e.wires.data(),
+                               e.witnesses.size(), e.pi_idx.data(), e.pi_idx.size(), hades, nullptr, 0, &n));
+  std::vector<uint8_t> out(n);
+  check(pb200_circuit_compress(e.n_constraints, e.selectors.empty() ? nullptr : e.selectors[0].data(), e.wires.data(),
+                               e.witnesses.size(), e.pi_idx.data(), e.pi_idx.size(), hades, out.data(), n, &n));
+  return out;
+}
 
 }  // namespace plonk_b200

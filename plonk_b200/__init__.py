@@ -6,10 +6,11 @@ Host-side mirror of the reference's crate-private seam (SURVEY.md section 8b):
     CommitKey.commit                                      reference src/commitment_scheme/kzg10/key.rs:376-388
     PublicParameters.setup / from_slice                   reference src/commitment_scheme/kzg10/srs.rs:61-178
     Compiler.compile / compile_with_circuit               reference src/compiler.rs:116-461
+    Compiler.compile_with_compressed, compress            reference src/compiler.rs:84-112, src/composer/circuit.rs:28-45
 
 Everything computes on the GPU through the C ABI in include/plonk_b200.h; there is no CPU path."""
 from ._lib import Pb200Error, PlonkVersion, lib  # noqa: F401
-from .compiler import Compiler, TruncatedDegreeTooLarge  # noqa: F401
+from .compiler import BlsScalarMalformed, Compiler, InvalidCompressedCircuit, TruncatedDegreeTooLarge, compress, compress_arrays  # noqa: F401
 from .domain import EvaluationDomain  # noqa: F401
 from .kzg import CommitKey, Commitment, PolynomialDegreeTooLarge  # noqa: F401
 from .prover import CircuitUnsatisfied, Prover, UnsupportedProvingVersion  # noqa: F401

@@ -21,6 +21,8 @@ PB200_ERR_POINT_MALFORMED = -10
 PB200_ERR_VERIFY = -11
 PB200_ERR_UNSUPPORTED_VERSION = -12
 PB200_ERR_DEGREE_IS_ZERO = -13
+PB200_ERR_INVALID_COMPRESSED = -14
+PB200_ERR_SCALAR_MALFORMED = -15
 
 
 class PlonkVersion(enum.IntEnum):
@@ -44,6 +46,7 @@ EXPORTS = [
     "pb200_g1_compress", "pb200_g1_compress_batch", "pb200_g1_decompress", "pb200_raw_commit_key_points", "pb200_commit_key_from_raw_var_bytes",
     "pb200_commit_key_to_raw_var_bytes", "pb200_prover_to_bytes", "pb200_g1_add_affine", "pb200_srs_setup_from_secret", "pb200_g1_lagrange_key",
     "pb200_public_parameters_setup", "pb200_opening_key_check",
+    "pb200_circuit_compress", "pb200_compressed_circuit_info", "pb200_prover_from_compressed",
     "pb200_profile_enable", "pb200_throughput_mode", "pb200_profile_read", "pb200_profile_read_sparse",
     "pb200_prover_new", "pb200_prover_from_bytes", "pb200_prover_free", "pb200_prover_commitments", "pb200_prove", "pb200_prove_dev",
     "pb200_prove_with_version", "pb200_prove_dev_with_version",
@@ -128,6 +131,11 @@ def lib() -> ctypes.CDLL:
         L.pb200_srs_setup_from_secret.argtypes = [c.c_void_p, c.c_void_p, c.c_size_t, c.c_void_p]
         L.pb200_public_parameters_setup.argtypes = [c.c_size_t, c.c_void_p, c.c_void_p, c.c_void_p, c.c_void_p, c.c_void_p]
         L.pb200_opening_key_check.argtypes = [c.c_void_p]
+        L.pb200_circuit_compress.argtypes = [c.c_size_t, c.c_void_p, c.c_void_p, c.c_size_t, c.c_void_p, c.c_size_t, c.c_int, c.c_void_p,
+                                             c.c_size_t, c.POINTER(c.c_size_t)]
+        L.pb200_compressed_circuit_info.argtypes = [c.c_void_p, c.c_size_t, c.c_size_t, c.POINTER(c.c_size_t), c.POINTER(c.c_uint64),
+                                                    c.POINTER(c.c_size_t), c.POINTER(c.c_size_t), c.c_void_p]
+        L.pb200_prover_from_compressed.argtypes = [c.c_void_p, c.c_size_t, c.c_void_p, c.c_size_t, c.c_void_p, c.c_size_t, c.POINTER(c.c_void_p)]
         L.pb200_profile_enable.argtypes = [c.c_int]
         L.pb200_throughput_mode.argtypes = [c.c_int]
         L.pb200_profile_read.argtypes = [c.POINTER(c.c_double), c.POINTER(c.c_uint64), c.POINTER(c.c_uint64), c.POINTER(c.c_uint64)]

@@ -21,6 +21,7 @@
 #include <mutex>
 #include <vector>
 
+#include "compress.h"
 #include "internal.cuh"
 #include "host_field.h"
 #include "plonk_algebra.cuh"
@@ -73,6 +74,26 @@ __global__ void k_gather_wires(const uint4* wit, const uint32_t* wires, size_t c
   Fr v = Fr::zero();
   if (i < constraints) v = ldg_fr(wit, wires[k * constraints + i]);
   stg_fr(out, (size_t)k * n + i, v);
+}
+
+// Selector columns of a compressed circuit (Compiler::compile_with_compressed): column k of gate i is
+// scalars[polys[11 * gate_poly[i] + k]], zero from the gate count up to n.  cols is [11][n], grid.y = 11.
+__global__ void k_expand_selectors(const uint4* __restrict__ scalars, const uint32_t* __restrict__ polys,
+                                   const uint32_t* __restrict__ gate_poly, size_t constraints, size_t n, uint4* cols) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const unsigned k = blockIdx.y;
+  Fr v = Fr::zero();
+  if (i < constraints) v = ldg_fr(scalars, __ldg(polys + (size_t)pbz::kSelectors * __ldg(gate_poly + i) + k));
+  stg_fr(cols, (size_t)k * n + i, v);
+}
+
+// The dense witness table of a compressed circuit's prover: dense[j] = wit[labels[j]] (the circuit's own numbering ->
+// the dense ids its wires use).
+__global__ void k_gather_witnesses(const uint4* __restrict__ wit, const unsigned long long* __restrict__ labels, size_t n_labels,
+                                   uint4* dense) {
+  const size_t j = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j < n_labels) stg_fr(dense, j, ldg_fr(wit, __ldg(labels + j)));
 }
 
 // coeffs[i] -= b_i ; coeffs[n + i] = b_i  (Prover::blind_poly_with_blinders, prover.rs:139-152)
@@ -560,6 +581,9 @@ struct pb200_prover {
   int has_widget[4] = {0, 0, 0, 0};
   uint8_t comm[pb::N_POLY][48];
   size_t n_witnesses = 0;
+  // a prover from a compressed circuit: the wires hold dense ids, labels[id] is the circuit's witness index
+  unsigned long long* d_labels = nullptr;
+  size_t n_labels = 0;
   // scratch arenas, one per proof in flight (allocated on first use, then recycled)
   mutable std::mutex ws_mu;
   mutable std::vector<pb::Arena> ws_free;
@@ -644,9 +668,12 @@ struct LoadedProverKey {
   uint8_t comm[N_POLY][48];
 };
 
+// selectors / wires / n_witnesses: the circuit as pb200_prover_new takes it.  loaded: a key read by
+// pb200_prover_from_bytes.  comp: a compressed circuit (selectors unused, wires = comp's dense ids, n_witnesses = the
+// circuit's own witness count); its selector columns are expanded on the device.
 static int prover_build(pb200_prover* P, const uint8_t* label, size_t label_len, size_t constraints, const uint64_t* selectors,
                         const uint32_t* wires, size_t n_witnesses, const uint8_t* srs_raw, size_t n_srs, cudaStream_t st,
-                        const LoadedProverKey* loaded = nullptr) {
+                        const LoadedProverKey* loaded = nullptr, const pbz::CompressedDescription* comp = nullptr) {
   P->label.assign(label, label + label_len);
   P->constraints = constraints;
   P->n_witnesses = n_witnesses;
@@ -728,15 +755,42 @@ static int prover_build(pb200_prover* P, const uint8_t* label, size_t label_len,
     PoolBlock cols_block(st);
     PB_CUDA(cols_block.alloc((size_t)N_POLY * n * 32));
     uint4* cols = (uint4*)cols_block.p;
-    PB_CUDA(cudaMemsetAsync(cols, 0, (size_t)N_POLY * n * 32, st));
-    PB_CUDA(cudaMemcpy2DAsync(cols, n * 32, selectors, constraints * 32, constraints * 32, 11, cudaMemcpyHostToDevice, st));
+    if (!comp) {
+      PB_CUDA(cudaMemsetAsync(cols, 0, (size_t)N_POLY * n * 32, st));
+      PB_CUDA(cudaMemcpy2DAsync(cols, n * 32, selectors, constraints * 32, constraints * 32, 11, cudaMemcpyHostToDevice, st));
+    } else {
+      // the scalar table (canonical -> Montgomery on the device), the polynomial table and one index per gate go up;
+      // k_expand_selectors writes all 11 x n selector entries and k_sigma_lagrange below the 4 x n sigma ones
+      const size_t n_sc = comp->scalars.size() / 32, n_pw = comp->polynomials.size();
+      PoolBlock tab_block(st);
+      PB_CUDA(tab_block.alloc(Arena::round_up(n_sc * 32) + Arena::round_up(n_pw * 4) + constraints * 4 + 4));
+      uint4* d_sc = (uint4*)tab_block.p;
+      uint32_t* d_pw = (uint32_t*)((char*)tab_block.p + Arena::round_up(n_sc * 32));
+      uint32_t* d_gp = d_pw + Arena::round_up(n_pw * 4) / 4;
+      unsigned* d_flag = d_gp + constraints;
+      PB_CUDA(cudaMemcpyAsync(d_sc, comp->scalars.data(), n_sc * 32, cudaMemcpyHostToDevice, st));
+      PB_CUDA(cudaMemcpyAsync(d_pw, comp->polynomials.data(), n_pw * 4, cudaMemcpyHostToDevice, st));
+      PB_CUDA(cudaMemcpyAsync(d_gp, comp->gate_poly.data(), constraints * 4, cudaMemcpyHostToDevice, st));
+      PB_CUDA(cudaMemsetAsync(d_flag, 0, 4, st));
+      PB_LAUNCH(k_fr_from_canonical, div_up(n_sc, 256), 256, 0, st, d_sc, n_sc, d_flag);
+      PB_LAUNCH(k_expand_selectors, dim3(div_up(n, 256), pbz::kSelectors), 256, 0, st, (const uint4*)d_sc, (const uint32_t*)d_pw,
+                (const uint32_t*)d_gp, constraints, n, cols);
+      unsigned h_flag = 0;
+      PB_CUDA(cudaMemcpyAsync(&h_flag, d_flag, 4, cudaMemcpyDeviceToHost, st));
+      PB_CUDA(cudaStreamSynchronize(st));  // the host tables must outlive the copies
+      if (h_flag) return fail(PB200_ERR_SCALAR_MALFORMED, "BlsScalarMalformed: a compressed circuit's scalar is not canonical");
+      PB_CUDA(cudaMalloc((void**)&P->d_labels, comp->labels.size() * 8));
+      PB_CUDA(cudaMemcpy(P->d_labels, comp->labels.data(), comp->labels.size() * 8, cudaMemcpyHostToDevice));
+      P->n_labels = comp->labels.size();
+    }
     // sigma permutation on the host (composer/permutation.rs:106-141), Lagrange values on the device
     {
-      std::vector<std::vector<uint64_t>> wmap(n_witnesses);
+      const size_t n_ids = comp ? comp->labels.size() : n_witnesses;  // the dense ids of a compressed circuit
+      std::vector<std::vector<uint64_t>> wmap(n_ids);
       for (size_t g = 0; g < constraints; g++)
         for (int k = 0; k < 4; k++) {
           const uint32_t w = wires[(size_t)k * constraints + g];
-          if (w >= n_witnesses) {
+          if (w >= n_ids) {
             return fail(PB200_ERR_INVALID_ARG, "wire index out of range");
           }
           wmap[w].push_back(((uint64_t)k << 40) | g);
@@ -831,6 +885,7 @@ static int prover_build(pb200_prover* P, const uint8_t* label, size_t label_len,
     proof_buffers(n, bytes);
     P->ws_bytes = call;
     for (size_t b : bytes) P->ws_bytes += Arena::round_up(b);
+    P->ws_bytes += Arena::round_up(P->n_labels * 32);  // the dense witness table of a compressed circuit
   }
   return 0;
 }
@@ -842,6 +897,24 @@ int prover_new(const uint8_t* label, size_t label_len, size_t constraints, const
   const int rc = prover_build(P, label, label_len, constraints, selectors, wires, n_witnesses, srs_raw, n_srs, thread_stream());
   if (rc != 0) {
     prover_free(P);  // releases whatever had been allocated; the error message is already set
+    return rc;
+  }
+  *out = P;
+  return 0;
+}
+
+// Compiler::compile_with_compressed's Prover (compiler.rs:84-112): the description decoded on the host, its selector
+// columns expanded on the device.
+int prover_from_compressed(const uint8_t* label, size_t label_len, const uint8_t* bytes, size_t len, const uint8_t* srs_raw,
+                           size_t n_srs, pb200_prover** out) {
+  pbz::CompressedDescription d;
+  PB_TRY(pbz::decode(bytes, len, n_srs, &d));
+  if (d.gates() == 0) return fail(PB200_ERR_INVALID_ARG, "empty circuit");
+  pb200_prover* P = new pb200_prover();
+  const int rc = prover_build(P, label, label_len, d.gates(), nullptr, d.wires.data(), (size_t)d.witnesses, srs_raw, n_srs,
+                              thread_stream(), nullptr, &d);
+  if (rc != 0) {
+    prover_free(P);
     return rc;
   }
   *out = P;
@@ -1117,6 +1190,7 @@ void prover_free(pb200_prover* P) {
   if (P->srs) srs_free(P->srs);
   if (P->srs_lag) srs_free(P->srs_lag);
   cudaFree(P->d_wires); cudaFree(P->d_polys); cudaFree(P->d_key8); cudaFree(P->d_linear8); cudaFree(P->d_l1_8); cudaFree(P->d_sigma);
+  cudaFree(P->d_labels);
   for (char* w : P->ws_all) cudaFree(w);
   delete P;
 }
@@ -1201,6 +1275,14 @@ int prove_dev(const pb200_prover* P, int version, const uint64_t* d_wit, const u
   uint64_t aff[4 * 12];
   uint8_t c48[N_COMM][48];
   Challenges ch;
+
+  if (P->d_labels) {  // a compressed circuit's prover: its wires index the dense table of the labels they use
+    uint4* dense = nullptr;
+    PB_ALLOC(scope, dense, P->n_labels * 32);
+    PB_LAUNCH(k_gather_witnesses, div_up(P->n_labels, 256), 256, 0, st, (const uint4*)d_wit, (const unsigned long long*)P->d_labels,
+              P->n_labels, dense);
+    d_wit = (const uint64_t*)dense;
+  }
 
   // ---- round 1 -------------------------------------------------------------------------------
   PB_LAUNCH(k_gather_wires, dim3(div_up(n, 256), 4), 256, 0, st, (const uint4*)d_wit, (const uint32_t*)P->d_wires, P->constraints, n, wv);
@@ -1474,6 +1556,13 @@ int pb200_prover_new(const uint8_t* label, size_t label_len, size_t n_constraint
   PB_TRY(ensure_init());
   if (!selectors || !wires || !srs_raw || !out) return fail(PB200_ERR_INVALID_ARG, "null argument");
   return prover_new(label, label_len, n_constraints, selectors, wires, n_witnesses, srs_raw, n_srs_points, out);
+}
+
+int pb200_prover_from_compressed(const uint8_t* label, size_t label_len, const uint8_t* bytes, size_t len,
+                                 const uint8_t* srs_raw, size_t n_srs_points, pb200_prover_t** out) {
+  if ((!label && label_len) || !bytes || !srs_raw || !out) return fail(PB200_ERR_INVALID_ARG, "null argument");
+  PB_TRY(ensure_init());
+  return prover_from_compressed(label, label_len, bytes, len, srs_raw, n_srs_points, out);
 }
 
 int pb200_throughput_mode(int on) {

@@ -21,6 +21,19 @@ class UnsupportedProvingVersion(ValueError):
     """Error::UnsupportedProvingVersion: PlonkVersion::V1 proofs cannot be made (reference prover.rs:376)."""
 
 
+def compressed_circuit_info(compressed: bytes, n_srs_points: int):
+    """pb200_compressed_circuit_info: (constraints, witnesses, labels, public-input count, public-input positions as
+    little-endian u64) of a compressed circuit, decoded within the bounds of public parameters of n_srs_points points.
+    Raises Pb200Error (PB200_ERR_INVALID_COMPRESSED or PB200_ERR_SCALAR_MALFORMED) for a description they reject."""
+    n, nw, nl, npi = ctypes.c_size_t(), ctypes.c_uint64(), ctypes.c_size_t(), ctypes.c_size_t()
+    args = (compressed, len(compressed), n_srs_points, ctypes.byref(n), ctypes.byref(nw), ctypes.byref(nl), ctypes.byref(npi))
+    check(lib().pb200_compressed_circuit_info(*args, None))
+    idx = ctypes.create_string_buffer(max(1, npi.value) * 8)
+    if npi.value:
+        check(lib().pb200_compressed_circuit_info(*args, idx))
+    return n.value, nw.value, nl.value, npi.value, idx.raw[: 8 * npi.value]
+
+
 class Prover:
     def __init__(self, label: bytes, n_constraints: int, selectors: bytes, wires: bytes, n_witnesses: int, srs_raw: bytes):
         assert len(selectors) == 11 * n_constraints * 32 and len(wires) == 4 * n_constraints * 4
@@ -40,6 +53,21 @@ class Prover:
         check(lib().pb200_prover_from_bytes(prover_bytes, len(prover_bytes), wires, n_witnesses, ctypes.byref(h)))
         self._h = h
         self.n_constraints = len(wires) // 16
+        self.n_witnesses = n_witnesses
+        return self
+
+    @classmethod
+    def from_compressed(cls, label: bytes, compressed: bytes, srs_raw: bytes, info=None) -> "Prover":
+        """The Prover of Compiler::compile_with_compressed (compiler.rs:84-112): the selector columns are expanded on the
+        GPU from the description's tables.  prove takes the re-run circuit's witness table, as for any Prover.  info: what
+        compressed_circuit_info returned for these bytes and keys, if the caller has it already."""
+        n_constraints, n_witnesses, _, _, _ = info or compressed_circuit_info(compressed, len(srs_raw) // 96)
+        self = cls.__new__(cls)
+        h = ctypes.c_void_p()
+        check(lib().pb200_prover_from_compressed(label, len(label), compressed, len(compressed), srs_raw, len(srs_raw) // 96,
+                                                 ctypes.byref(h)))
+        self._h = h
+        self.n_constraints = n_constraints
         self.n_witnesses = n_witnesses
         return self
 
