@@ -32,6 +32,8 @@
  *                                    src/composer/circuit.rs:28-45, src/composer/compress.rs:136-240
  *   pb200_compressed_circuit_info / pb200_prover_from_compressed
  *                                    Compiler::compile_with_compressed   src/compiler.rs:84-112, compress.rs:242-461
+ *   pb200_circuit_unsatisfied / pb200_prover_unsatisfied / pb200_identity_family
+ *                                    Debugger::unsatisfied_constraints / unsatisfied_report   src/debugger.rs:31-236
  *   (Compiler::compile, src/compiler.rs:116-461, is pb200_prover_new, pb200_prover_commitments and pb200_verifier_new
  *    in sequence; the mirrors write it once.)
  *
@@ -293,6 +295,43 @@ int pb200_prove_with_version(const pb200_prover_t* prover, int version, const ui
 int pb200_prove_dev_with_version(const pb200_prover_t* prover, int version, const uint64_t* d_witnesses, size_t n_witnesses,
                                  const uint64_t* pi_idx, const uint64_t* pi_vals, size_t n_pi,
                                  const uint64_t* blinders, uint8_t* out_proof, void* stream);
+
+/* ---- which constraint a witness breaks (the reference's debugger, src/debugger.rs:31-236) ------------------------- */
+/* IDENTITY_FAMILIES[k] of the reference (debugger.rs:31-49), k = 0..16: "arithmetic", the four range identities
+ * ("range delta c/d", "range delta b/c", "range delta a/b", "range accumulator"), the five logic ones ("logic left
+ * quad", "logic right quad", "logic output quad", "logic product", "logic relation"), the four fixed-base ones
+ * ("fixed-base bit consistency", "fixed-base xy consistency", "fixed-base x accumulator", "fixed-base y accumulator")
+ * and the three variable-base ones ("variable-base xy consistency", "variable-base x accumulator", "variable-base y
+ * accumulator").  NULL for any other k.  No device needed. */
+const char* pb200_identity_family(int k);
+/* Debugger::unsatisfied_constraints (debugger.rs:95-205) on the GPU: every constraint's 17 gate identities, evaluated
+ * in that order, with a_w, b_w and d_w read from row (i + 1) mod next_pow2(n_constraints) and as zero from a padding
+ * row (the prover's cyclic domain).  An identity fails when it is not zero mod r; each widget identity is taken times
+ * its selector, and the public input is added to the arithmetic identity outside q_arith.  This call checks a circuit
+ * as pb200_prover_new takes it (selectors, wires) with its witness table and public inputs: what the composer holds at
+ * prove time, which is what the reference's debugger checks.  No public parameters are needed.
+ *   *n_unsatisfied always receives the number of failing constraints; rows / families receive the first min(cap, that
+ *   number) of them in ascending row order, each with the index k of the first identity it fails
+ *   (pb200_identity_family(k)).  With cap = 0, rows and families may be NULL.
+ *   PB200_ERR_INVALID_ARG: a NULL array that is needed, public inputs that pb200_prove would refuse (positions outside
+ *   the circuit or not strictly increasing), a wire index >= n_witnesses (as for pb200_prover_new).
+ *   n_constraints = 0 is PB200_OK with a count of 0.
+ * The call does not change when pb200_prove returns PB200_ERR_UNSATISFIED, and it checks no copy constraints: wires
+ * are witness indices, so those always hold. */
+int pb200_circuit_unsatisfied(size_t n_constraints, const uint64_t* selectors, const uint32_t* wires,
+                              const uint64_t* witnesses, size_t n_witnesses,
+                              const uint64_t* pi_idx, const uint64_t* pi_vals, size_t n_pi,
+                              size_t cap, uint64_t* rows, int32_t* families, size_t* n_unsatisfied);
+/* The same identities against the compiled prover's own selectors, with exactly the inputs pb200_prove takes (n_witnesses
+ * must be the prover's): what a proof enforces.  The selector values come from one forward NTT of the prover's key, so
+ * this works for provers from pb200_prover_new, pb200_prover_from_bytes and pb200_prover_from_compressed.  Outputs and
+ * argument checks as pb200_circuit_unsatisfied.  The call reads only what a prover never changes and runs on the
+ * calling thread's pb200 stream, so it may run beside proofs on the same prover.  When the circuit a witness was made
+ * with sets a selector the compiled one does not, pb200_circuit_unsatisfied can name a row that this call, and the
+ * proof, accept; when this call reports nothing, pb200_prove makes the proof. */
+int pb200_prover_unsatisfied(const pb200_prover_t* prover, const uint64_t* witnesses, size_t n_witnesses,
+                             const uint64_t* pi_idx, const uint64_t* pi_vals, size_t n_pi,
+                             size_t cap, uint64_t* rows, int32_t* families, size_t* n_unsatisfied);
 
 /* ---- compressed circuits (Circuit::compress, Compiler::compile_with_compressed) ----------------------------------- */
 /* CompressedCircuit::from_composer (src/composer/compress.rs:136-240; Circuit::compress, circuit.rs:28-45): the circuit

@@ -17,6 +17,8 @@
 //   plonk_b200::Compiler           src/compiler.rs:47-113, 116-461                     compile, compile_with_circuit,
 //                                                                                      compile_with_compressed
 //   plonk_b200::compress           src/composer/circuit.rs:28-45, src/composer/compress.rs:136-240   Circuit::compress
+//   plonk_b200::unsatisfied_constraints / unsatisfied_report, Prover::unsatisfied_constraints / _report
+//                                  src/debugger.rs:95-236 (the report without its "appended at" clause)
 //   plonk_b200::Composer           src/composer.rs:72-495 + src/composer/{bits,range,logic,truncate,select,
 //                                  point,fixed_base}.rs (host-side circuit front end, plonk_b200_composer.h)
 //   plonk_b200::Error              src/error.rs:21-120 (the variants this path can produce)
@@ -30,6 +32,7 @@
 #include <cstdint>
 #include <stdexcept>
 #include <memory>
+#include <optional>
 #include <string>
 #include <utility>
 #include <vector>
@@ -362,6 +365,51 @@ inline Circuit circuit_of(const Composer::Export& e) {
   return c;
 }
 
+// ---- which constraint a witness breaks (the reference's debugger, src/debugger.rs:95-236) --------------------------
+// A failing constraint and the name of the first of its 17 gate identities that is not zero (IDENTITY_FAMILIES).
+using Unsatisfied = std::vector<std::pair<uint64_t, std::string>>;
+
+namespace detail {
+// call(cap, rows, families, &n): one of the C entry points with its circuit arguments bound.  Returns the failing count
+// and the first min(cap, count) failing constraints.
+template <class F>
+inline std::pair<size_t, Unsatisfied> unsatisfied_query(F&& call, size_t cap) {
+  std::vector<uint64_t> rows(cap);
+  std::vector<int32_t> families(cap);
+  size_t n = 0;
+  check(call(cap, cap ? rows.data() : nullptr, cap ? families.data() : nullptr, &n));
+  Unsatisfied out;
+  for (size_t i = 0; i < std::min(cap, n); i++) out.emplace_back(rows[i], pb200_identity_family(families[i]));
+  return {n, out};
+}
+// Debugger::unsatisfied_report without its "and was appended at path:line:col" clause (no call sites are recorded)
+inline std::optional<std::string> unsatisfied_report(const std::pair<size_t, Unsatisfied>& q, size_t n_constraints) {
+  if (q.first == 0) return std::nullopt;
+  return "plonk debugger: " + std::to_string(q.first) + " of " + std::to_string(n_constraints) +
+         " constraints are unsatisfied; the first, constraint " + std::to_string(q.second[0].first) + ", fails the " +
+         q.second[0].second + " identity";
+}
+inline auto composer_call(const Composer::Export& e) {
+  return [&e](size_t cap, uint64_t* rows, int32_t* families, size_t* n) {
+    return pb200_circuit_unsatisfied(e.n_constraints, e.selectors.empty() ? nullptr : e.selectors[0].data(), e.wires.data(),
+                                     e.witnesses.empty() ? nullptr : e.witnesses[0].data(), e.witnesses.size(), e.pi_idx.data(),
+                                     e.pi_vals.empty() ? nullptr : e.pi_vals[0].data(), e.pi_idx.size(), cap, rows, families, n);
+  };
+}
+}  // namespace detail
+
+// The reference debugger's check of a filled composer (its constraints, witnesses and public inputs, as at prove time):
+// every failing constraint in ascending order.
+inline Unsatisfied unsatisfied_constraints(const Composer& composer) {
+  const Composer::Export e = composer.finish();
+  return detail::unsatisfied_query(detail::composer_call(e), e.n_constraints).second;
+}
+// Debugger::unsatisfied_report of a filled composer; nullopt when every constraint holds.
+inline std::optional<std::string> unsatisfied_report(const Composer& composer) {
+  const Composer::Export e = composer.finish();
+  return detail::unsatisfied_report(detail::unsatisfied_query(detail::composer_call(e), 1), e.n_constraints);
+}
+
 // PlonkVersion (src/compiler.rs:22-42): V3 is the current profile; V2 is the legacy transcript seed with V3's opening
 // checks; V1 is the legacy seed with the legacy opening, which does not bind the q_arith, q_c, q_l and q_r
 // evaluations, so a V1 verdict is meaningful only for proofs made under the old rules.
@@ -370,7 +418,8 @@ enum class PlonkVersion { V1 = PB200_PLONK_V1, V2 = PB200_PLONK_V2, V3 = PB200_P
 class Prover {
  public:
   static constexpr size_t PROOF_SIZE = 1008;  // Proof::SIZE
-  Prover(const std::string& label, const Circuit& c, const uint8_t* srs_raw, size_t n_srs_points) : n_witnesses_(c.n_witnesses) {
+  Prover(const std::string& label, const Circuit& c, const uint8_t* srs_raw, size_t n_srs_points)
+      : n_witnesses_(c.n_witnesses), n_constraints_(c.n_constraints) {
     check(pb200_prover_new((const uint8_t*)label.data(), label.size(), c.n_constraints, c.selectors[0].data(), c.wires.data(),
                            c.n_witnesses, srs_raw, n_srs_points, &h_));
   }
@@ -379,6 +428,7 @@ class Prover {
   static std::unique_ptr<Prover> try_from_bytes(const uint8_t* bytes, size_t len, const std::vector<uint32_t>& wires, size_t n_witnesses) {
     std::unique_ptr<Prover> p(new Prover());
     p->n_witnesses_ = n_witnesses;
+    p->n_constraints_ = wires.size() / 4;
     check(pb200_prover_from_bytes(bytes, len, wires.data(), n_witnesses, &p->h_));
     return p;
   }
@@ -388,6 +438,10 @@ class Prover {
                                                  size_t n_srs_points, size_t n_witnesses) {
     std::unique_ptr<Prover> p(new Prover());
     p->n_witnesses_ = n_witnesses;
+    uint64_t described_witnesses = 0;
+    size_t n_labels = 0, n_pi = 0;
+    check(pb200_compressed_circuit_info(compressed.data(), compressed.size(), n_srs_points, &p->n_constraints_, &described_witnesses,
+                                        &n_labels, &n_pi, nullptr));
     check(pb200_prover_from_compressed((const uint8_t*)label.data(), label.size(), compressed.data(), compressed.size(), srs_raw,
                                        n_srs_points, &p->h_));
     return p;
@@ -426,11 +480,32 @@ class Prover {
                                    pi_vals.empty() ? nullptr : pi_vals[0].data(), pi_idx.size(), blinders[0].data(), proof.data()));
     return proof;
   }
+  // The reference debugger's check (debugger.rs:95-205) against this prover's own selectors, with prove's arguments:
+  // every failing constraint in ascending order.  Empty means prove makes the proof.  Safe beside proofs on this prover.
+  Unsatisfied unsatisfied_constraints(const std::vector<BlsScalar>& witnesses, const std::vector<uint64_t>& pi_idx,
+                                      const std::vector<BlsScalar>& pi_vals) const {
+    return unsatisfied_query(witnesses, pi_idx, pi_vals, n_constraints_).second;
+  }
+  // Debugger::unsatisfied_report for unsatisfied_constraints; nullopt when every constraint holds.
+  std::optional<std::string> unsatisfied_report(const std::vector<BlsScalar>& witnesses, const std::vector<uint64_t>& pi_idx,
+                                                const std::vector<BlsScalar>& pi_vals) const {
+    return detail::unsatisfied_report(unsatisfied_query(witnesses, pi_idx, pi_vals, 1), n_constraints_);
+  }
 
  private:
-  Prover() : n_witnesses_(0) {}
+  Prover() : n_witnesses_(0), n_constraints_(0) {}
+  std::pair<size_t, Unsatisfied> unsatisfied_query(const std::vector<BlsScalar>& witnesses, const std::vector<uint64_t>& pi_idx,
+                                                   const std::vector<BlsScalar>& pi_vals, size_t cap) const {
+    return detail::unsatisfied_query(
+        [&](size_t c, uint64_t* rows, int32_t* families, size_t* n) {
+          return pb200_prover_unsatisfied(h_, witnesses.empty() ? nullptr : witnesses[0].data(), witnesses.size(), pi_idx.data(),
+                                          pi_vals.empty() ? nullptr : pi_vals[0].data(), pi_idx.size(), c, rows, families, n);
+        },
+        cap);
+  }
   pb200_prover_t* h_ = nullptr;
   size_t n_witnesses_;
+  size_t n_constraints_;
 };
 
 class Verifier;

@@ -7,9 +7,12 @@ Host-side mirror of the reference's crate-private seam (SURVEY.md section 8b):
     PublicParameters.setup / from_slice                   reference src/commitment_scheme/kzg10/srs.rs:61-178
     Compiler.compile / compile_with_circuit               reference src/compiler.rs:116-461
     Compiler.compile_with_compressed, compress            reference src/compiler.rs:84-112, src/composer/circuit.rs:28-45
+    unsatisfied_constraints / unsatisfied_report,         reference src/debugger.rs:95-236
+      Prover.unsatisfied_constraints / _report
 
 Everything computes on the GPU through the C ABI in include/plonk_b200.h; there is no CPU path."""
 from ._lib import Pb200Error, PlonkVersion, lib  # noqa: F401
+from .debugger import identity_family, unsatisfied_constraints, unsatisfied_report  # noqa: F401
 from .compiler import BlsScalarMalformed, Compiler, InvalidCompressedCircuit, TruncatedDegreeTooLarge, compress, compress_arrays  # noqa: F401
 from .domain import EvaluationDomain  # noqa: F401
 from .kzg import CommitKey, Commitment, PolynomialDegreeTooLarge  # noqa: F401

@@ -47,6 +47,7 @@ EXPORTS = [
     "pb200_commit_key_to_raw_var_bytes", "pb200_prover_to_bytes", "pb200_g1_add_affine", "pb200_srs_setup_from_secret", "pb200_g1_lagrange_key",
     "pb200_public_parameters_setup", "pb200_opening_key_check",
     "pb200_circuit_compress", "pb200_compressed_circuit_info", "pb200_prover_from_compressed",
+    "pb200_identity_family", "pb200_circuit_unsatisfied", "pb200_prover_unsatisfied",
     "pb200_profile_enable", "pb200_throughput_mode", "pb200_profile_read", "pb200_profile_read_sparse",
     "pb200_prover_new", "pb200_prover_from_bytes", "pb200_prover_free", "pb200_prover_commitments", "pb200_prove", "pb200_prove_dev",
     "pb200_prove_with_version", "pb200_prove_dev_with_version",
@@ -136,6 +137,12 @@ def lib() -> ctypes.CDLL:
         L.pb200_compressed_circuit_info.argtypes = [c.c_void_p, c.c_size_t, c.c_size_t, c.POINTER(c.c_size_t), c.POINTER(c.c_uint64),
                                                     c.POINTER(c.c_size_t), c.POINTER(c.c_size_t), c.c_void_p]
         L.pb200_prover_from_compressed.argtypes = [c.c_void_p, c.c_size_t, c.c_void_p, c.c_size_t, c.c_void_p, c.c_size_t, c.POINTER(c.c_void_p)]
+        L.pb200_identity_family.argtypes = [c.c_int]
+        L.pb200_identity_family.restype = c.c_char_p
+        L.pb200_circuit_unsatisfied.argtypes = [c.c_size_t, c.c_void_p, c.c_void_p, c.c_void_p, c.c_size_t, c.c_void_p, c.c_void_p,
+                                                c.c_size_t, c.c_size_t, c.c_void_p, c.c_void_p, c.POINTER(c.c_size_t)]
+        L.pb200_prover_unsatisfied.argtypes = [c.c_void_p, c.c_void_p, c.c_size_t, c.c_void_p, c.c_void_p, c.c_size_t, c.c_size_t,
+                                               c.c_void_p, c.c_void_p, c.POINTER(c.c_size_t)]
         L.pb200_profile_enable.argtypes = [c.c_int]
         L.pb200_throughput_mode.argtypes = [c.c_int]
         L.pb200_profile_read.argtypes = [c.POINTER(c.c_double), c.POINTER(c.c_uint64), c.POINTER(c.c_uint64), c.POINTER(c.c_uint64)]

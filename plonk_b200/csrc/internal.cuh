@@ -56,6 +56,12 @@ int lagrange_key_dev(const uint4* d_in, int log_n, uint4* d_out, cudaStream_t st
 int opening_key_check(const uint8_t* opening_key);
 int opening_key_g2(const uint64_t* x_mont, const uint64_t* h_scalar_mont, uint8_t* out_2x96);
 
+// debugger.cu: the reference debugger's row check over columns already on the device (sel [11][n] selector values,
+// wv [4][n] wire values zero-padded past the constraints, pi [n] or null); writes the total to *n_unsatisfied and the
+// first min(cap, total) failing rows and their identity indices to the host arrays rows / families.  Synchronises st.
+int unsatisfied_run(const uint4* sel, const uint4* wv, const uint4* pi, size_t n, size_t constraints, size_t cap, uint64_t* rows,
+                    int32_t* families, size_t* n_unsatisfied, cudaStream_t st);
+
 // capi.cu
 int raw_commit_key_parse(const uint8_t* bytes, size_t len, int checked, size_t* n_points, uint8_t* out_raw);
 void raw_commit_key_record(const uint8_t* raw96, uint8_t* rec97);

@@ -151,6 +151,85 @@ PB_HD F widget_var(const SepPowers<S>& s, const F& ed, const WireVals<F>& v) {  
   return (xy + x3c + y3c) * ch;
 }
 
+// ---- gate identities, one per row (debugger.rs:31-49, 95-180) ------------------------------------------------
+// The terms the widgets above combine, one by one and without their separation challenge: each widget is ch times
+// the kappa-weighted sum of its terms, in the order below (kappa^j weights term j; the fixed-base widget's terms in
+// this order are bit, xy kappa, x kappa^2, y kappa^3).  tests/test_debugger_algebra.py checks that relation.  The
+// 17 identities of a row are the arithmetic term plus these terms, each times its widget's selector.
+enum IdentityFamily { ID_ARITH = 0, ID_RANGE = 1, ID_LOGIC = 5, ID_FIXED = 10, ID_VAR = 14, N_IDENTITIES = 17 };
+static const char* const kIdentityFamilies[N_IDENTITIES] = {
+    "arithmetic",
+    "range delta c/d", "range delta b/c", "range delta a/b", "range accumulator",
+    "logic left quad", "logic right quad", "logic output quad", "logic product", "logic relation",
+    "fixed-base bit consistency", "fixed-base xy consistency", "fixed-base x accumulator", "fixed-base y accumulator",
+    "variable-base xy consistency", "variable-base x accumulator", "variable-base y accumulator"};
+
+template <class F, int K>
+struct Terms {
+  F t[K];
+};
+// q(k) returns the selector k (Poly order) of the row
+PB_HOST_INSTANTIABLE
+template <class F, class Sel>
+PB_HD F arith_identity(const Sel& q, const F& pi, const WireVals<F>& v) {  // arithmetic/proverkey.rs:44-69
+  return (v.a * v.b * q(Q_M) + v.a * q(Q_L) + v.b * q(Q_R) + v.c * q(Q_O) + v.d * q(Q_F) + q(Q_C)) * q(Q_ARITH) + pi;
+}
+PB_HOST_INSTANTIABLE
+template <class F>
+PB_HD Terms<F, 4> range_terms(const WireVals<F>& v) {
+  return {{delta4(v.c - mul_small(v.d, 4)), delta4(v.b - mul_small(v.c, 4)), delta4(v.a - mul_small(v.b, 4)), delta4(v.d_w - mul_small(v.a, 4))}};
+}
+PB_HOST_INSTANTIABLE
+template <class F>
+PB_HD Terms<F, 5> logic_terms(const F& q_c, const WireVals<F>& v) {
+  const F A = v.a_w - mul_small(v.a, 4), B = v.b_w - mul_small(v.b, 4), D = v.d_w - mul_small(v.d, 4);
+  const F& w = v.c;
+  const F ab = A + B;
+  const F Fx = w * (w * (mul_small(w, 4) - mul_small(ab, 18) + mul_small(F::one(), 81)) + mul_small(A.sqr() + B.sqr(), 18) - mul_small(ab, 81) + mul_small(F::one(), 83));
+  const F E = mul_small(ab + D, 3) - Fx.dbl();
+  const F Bq = q_c * (mul_small(D, 9) - mul_small(ab, 3));
+  return {{delta4(A), delta4(B), delta4(D), w - A * B, Bq + E}};
+}
+PB_HOST_INSTANTIABLE
+template <class F>
+PB_HD Terms<F, 4> fixed_terms(const F& ed, const F& q_l, const F& q_r, const F& q_c, const WireVals<F>& v) {
+  const F one = F::one();
+  const F bit = v.d_w - v.d - v.d;
+  const F y_alpha = bit.sqr() * (q_r - one) + one, x_alpha = bit * q_l;
+  const F t = v.c * v.a * v.b * ed;
+  return {{bit * (bit - one) * (bit + one), bit * q_c - v.c, (v.a_w + v.a_w * t) - (v.a * y_alpha + v.b * x_alpha),
+           (v.b_w - v.b_w * t) - (v.b * y_alpha + v.a * x_alpha)}};
+}
+PB_HOST_INSTANTIABLE
+template <class F>
+PB_HD Terms<F, 3> var_terms(const F& ed, const WireVals<F>& v) {
+  const F &x1 = v.a, &x3 = v.a_w, &y1 = v.b, &y3 = v.b_w, &x2 = v.c, &y2 = v.d, &x1y2 = v.d_w;
+  const F y1x2 = y1 * x2;
+  const F t = ed * x1y2 * y1x2;
+  return {{x1 * y2 - x1y2, (x1y2 + y1x2) - (x3 + x3 * t), (y1 * y2 + x1 * x2) - (y3 - y3 * t)}};
+}
+PB_HOST_INSTANTIABLE
+template <class F, int K>
+PB_HD int first_nonzero(const Terms<F, K>& t, int family) {
+  for (int k = 0; k < K; k++)
+    if (!t.t[k].is_zero()) return family + k;
+  return -1;
+}
+// The index (IdentityFamily + term) of the first of the row's 17 identities that is not zero, or -1.  A term times a
+// non-zero selector is zero exactly when the term is, so a widget whose selector is zero is skipped and the others are
+// tested without the product; the arithmetic identity is skipped only when both q_arith and pi are zero.
+PB_HOST_INSTANTIABLE
+template <class F, class Sel>
+PB_HD int first_failing_identity(const Sel& q, const F& pi, const F& ed, const WireVals<F>& v) {
+  int r = -1;
+  if ((!q(Q_ARITH).is_zero() || !pi.is_zero()) && !arith_identity(q, pi, v).is_zero()) return ID_ARITH;
+  if (!q(Q_RANGE).is_zero() && (r = first_nonzero(range_terms(v), ID_RANGE)) >= 0) return r;
+  if (!q(Q_LOGIC).is_zero() && (r = first_nonzero(logic_terms(q(Q_C), v), ID_LOGIC)) >= 0) return r;
+  if (!q(Q_FIXED).is_zero() && (r = first_nonzero(fixed_terms(ed, q(Q_L), q(Q_R), q(Q_C), v), ID_FIXED)) >= 0) return r;
+  if (!q(Q_VAR).is_zero() && (r = first_nonzero(var_terms(ed, v), ID_VAR)) >= 0) return r;
+  return -1;
+}
+
 // ---- permutation (permutation/proverkey.rs:40-125) -----------------------------------------------------------
 // The identity permutation's product at a point x, with bx = beta x and the coset constants K1..K3 = 7, 13, 17:
 // (a + bx + gamma)(b + 7 bx + gamma)(c + 13 bx + gamma)(d + 17 bx + gamma).

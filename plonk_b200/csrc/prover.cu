@@ -1195,6 +1195,17 @@ void prover_free(pb200_prover* P) {
   delete P;
 }
 
+// The public inputs of a proof: positions inside the circuit, strictly increasing (the reference keeps them in a
+// BTreeMap keyed by gate index, composer.rs:465-480: ascending, no duplicates).
+static int check_public_inputs(const uint64_t* pi_idx, const uint64_t* pi_vals, size_t n_pi, size_t constraints) {
+  if (n_pi && (!pi_idx || !pi_vals)) return fail(PB200_ERR_INVALID_ARG, "public inputs announced but not given");
+  for (size_t i = 0; i < n_pi; i++) {
+    if (pi_idx[i] >= constraints) return fail(PB200_ERR_INVALID_ARG, "public input index out of range");
+    if (i && pi_idx[i] <= pi_idx[i - 1]) return fail(PB200_ERR_INVALID_ARG, "public input positions must be strictly increasing");
+  }
+  return 0;
+}
+
 // Prover::prove_inner.  d_wit: n_witnesses Fr on the device; pi_*: host.  version: PB200_PLONK_V3 or V2, which read
 // the same except for the transcript seed (Prover::transcript_for_version, prover.rs:404-413).
 int prove_dev(const pb200_prover* P, int version, const uint64_t* d_wit, const uint64_t* pi_idx, const uint64_t* pi_vals,
@@ -1220,13 +1231,8 @@ int prove_dev(const pb200_prover* P, int version, const uint64_t* d_wit, const u
                            ? pbh::seed_transcript(P->label.data(), P->label.size(), P->constraints, P->comm[0], P->constraints)
                            : pbh::seed_transcript_legacy(P->label.data(), P->label.size(), P->constraints, P->comm[0], P->constraints);
   const HFr* PIV = (const HFr*)pi_vals;
-  if (n_pi && (!pi_idx || !pi_vals)) return fail(PB200_ERR_INVALID_ARG, "public inputs announced but not given");
-  for (size_t i = 0; i < n_pi; i++) {
-    if (pi_idx[i] >= P->constraints) return fail(PB200_ERR_INVALID_ARG, "public input index out of range");
-    // the reference keeps public inputs in a BTreeMap keyed by gate index (composer.rs:465-480): ascending, no duplicates
-    if (i && pi_idx[i] <= pi_idx[i - 1]) return fail(PB200_ERR_INVALID_ARG, "public input positions must be strictly increasing");
-    tr.append_scalar("pi", PIV[i]);
-  }
+  PB_TRY(check_public_inputs(pi_idx, pi_vals, n_pi, P->constraints));
+  for (size_t i = 0; i < n_pi; i++) tr.append_scalar("pi", PIV[i]);
   const uint4* w_half = nullptr;
   PB_TRY(get_twiddles(log_n, false, st, &w_half));
 
@@ -1544,6 +1550,25 @@ int prove_dev(const pb200_prover* P, int version, const uint64_t* d_wit, const u
   return 0;
 }
 
+// The debugger's check (debugger.cu) of a circuit whose selector values sel ([11][n]) are on the device: the wire values
+// are gathered from d_wit (the table d_wires indexes) and the dense public-input vector is built as prove_dev builds it.
+static int unsatisfied_columns(const uint4* sel, const uint4* d_wit, const uint32_t* d_wires, size_t constraints, size_t n,
+                               const uint64_t* pi_idx, const uint64_t* pi_vals, size_t n_pi, size_t cap, uint64_t* rows,
+                               int32_t* families, size_t* n_unsatisfied, cudaStream_t st) {
+  ScratchScope scope(nullptr, st);
+  uint4* wv = nullptr;
+  PB_ALLOC(scope, wv, (n_pi ? 5 : 4) * n * 32);
+  PB_LAUNCH(k_gather_wires, dim3(div_up(n, 256), 4), 256, 0, st, d_wit, d_wires, constraints, n, wv);
+  uint4* pi_dense = nullptr;
+  if (n_pi) {
+    pi_dense = wv + 2 * 4 * n;
+    PB_CUDA(cudaMemsetAsync(pi_dense, 0, n * 32, st));
+    for (size_t i = 0; i < n_pi; i++)
+      PB_CUDA(cudaMemcpyAsync(pi_dense + 2 * pi_idx[i], pi_vals + 4 * i, 32, cudaMemcpyHostToDevice, st));
+  }
+  return unsatisfied_run(sel, wv, pi_dense, n, constraints, cap, rows, families, n_unsatisfied, st);
+}
+
 }  // namespace pb
 
 using namespace pb;
@@ -1640,5 +1665,58 @@ int pb200_prove_dev_with_version(const pb200_prover_t* p, int version, const uin
   if (n_witnesses != p->n_witnesses) return fail(PB200_ERR_INVALID_ARG, "witness count differs from the compiled circuit");
   cudaStream_t st = stream ? (cudaStream_t)stream : thread_stream();
   return prove_dev(p, version, d_witnesses, pi_idx, pi_vals, n_pi, blinders, out_proof, st);
+}
+
+int pb200_circuit_unsatisfied(size_t n_constraints, const uint64_t* selectors, const uint32_t* wires, const uint64_t* witnesses,
+                              size_t n_witnesses, const uint64_t* pi_idx, const uint64_t* pi_vals, size_t n_pi, size_t cap,
+                              uint64_t* rows, int32_t* families, size_t* n_unsatisfied) {
+  if (!n_unsatisfied || (cap && (!rows || !families))) return fail(PB200_ERR_INVALID_ARG, "null argument");
+  PB_TRY(check_public_inputs(pi_idx, pi_vals, n_pi, n_constraints));
+  *n_unsatisfied = 0;
+  if (n_constraints == 0) return 0;  // the reference's debugger with no constraints reports nothing
+  if (!selectors || !wires || (n_witnesses && !witnesses)) return fail(PB200_ERR_INVALID_ARG, "null argument");
+  for (size_t j = 0; j < 4 * n_constraints; j++)
+    if (wires[j] >= n_witnesses) return fail(PB200_ERR_INVALID_ARG, "wire index out of range");
+  PB_TRY(ensure_init());
+  size_t n = 1;
+  while (n < n_constraints) n <<= 1;
+  cudaStream_t st = thread_stream();
+  ScratchScope scope(nullptr, st);
+  uint4 *sel = nullptr, *d_wit = nullptr;
+  uint32_t* d_wires = nullptr;
+  PB_ALLOC(scope, sel, (size_t)11 * n * 32);
+  PB_ALLOC(scope, d_wit, n_witnesses * 32);
+  PB_ALLOC(scope, d_wires, 4 * n_constraints * 4);
+  // only the rows below the constraint count are read, so the columns' padding is left as it is
+  PB_CUDA(cudaMemcpy2DAsync(sel, n * 32, selectors, n_constraints * 32, n_constraints * 32, 11, cudaMemcpyHostToDevice, st));
+  PB_CUDA(cudaMemcpyAsync(d_wit, witnesses, n_witnesses * 32, cudaMemcpyHostToDevice, st));
+  PB_CUDA(cudaMemcpyAsync(d_wires, wires, 4 * n_constraints * 4, cudaMemcpyHostToDevice, st));
+  return unsatisfied_columns(sel, d_wit, d_wires, n_constraints, n, pi_idx, pi_vals, n_pi, cap, rows, families, n_unsatisfied, st);
+}
+
+int pb200_prover_unsatisfied(const pb200_prover_t* p, const uint64_t* witnesses, size_t n_witnesses, const uint64_t* pi_idx,
+                             const uint64_t* pi_vals, size_t n_pi, size_t cap, uint64_t* rows, int32_t* families,
+                             size_t* n_unsatisfied) {
+  if (!p || !witnesses || !n_unsatisfied || (cap && (!rows || !families))) return fail(PB200_ERR_INVALID_ARG, "null argument");
+  if (n_witnesses != p->n_witnesses) return fail(PB200_ERR_INVALID_ARG, "witness count differs from the compiled circuit");
+  PB_TRY(check_public_inputs(pi_idx, pi_vals, n_pi, p->constraints));
+  PB_TRY(ensure_init());
+  const size_t n = p->n;
+  cudaStream_t st = thread_stream();
+  ScratchScope scope(nullptr, st);
+  uint4 *sel = nullptr, *d_wit = nullptr;
+  PB_ALLOC(scope, sel, (size_t)11 * n * 32);
+  PB_ALLOC(scope, d_wit, n_witnesses * 32);
+  // the selector values on the domain: one forward NTT of the key's 11 selector polynomials
+  PB_TRY(ntt_run((const uint64_t*)p->d_polys, n, (uint64_t*)sel, p->log_n, 0, 0, 11, n, n, st, nullptr));
+  PB_CUDA(cudaMemcpyAsync(d_wit, witnesses, n_witnesses * 32, cudaMemcpyHostToDevice, st));
+  if (p->d_labels) {  // a compressed circuit's prover: its wires index the dense table of the labels they use
+    uint4* dense = nullptr;
+    PB_ALLOC(scope, dense, p->n_labels * 32);
+    PB_LAUNCH(k_gather_witnesses, div_up(p->n_labels, 256), 256, 0, st, (const uint4*)d_wit, (const unsigned long long*)p->d_labels,
+              p->n_labels, dense);
+    d_wit = dense;
+  }
+  return unsatisfied_columns(sel, d_wit, p->d_wires, p->constraints, n, pi_idx, pi_vals, n_pi, cap, rows, families, n_unsatisfied, st);
 }
 }

@@ -8,6 +8,7 @@ from __future__ import annotations
 
 import ctypes
 
+from . import debugger
 from ._lib import PB200_ERR_UNSATISFIED, PB200_ERR_UNSUPPORTED_VERSION, Pb200Error, PlonkVersion, check, lib
 
 PROOF_BYTES = 1008
@@ -111,6 +112,23 @@ class Prover:
                 raise UnsupportedProvingVersion("UnsupportedProvingVersion") from e
             raise
         return out.raw
+
+    def _unsatisfied_call(self, witnesses: bytes, pi_idx: bytes, pi_vals: bytes):
+        assert len(witnesses) == self.n_witnesses * 32
+        return lambda cap, rows, fams, n: lib().pb200_prover_unsatisfied(self._h, witnesses, self.n_witnesses, pi_idx or None,
+                                                                        pi_vals or None, len(pi_idx) // 8, cap, rows, fams, n)
+
+    def unsatisfied_constraints(self, witnesses: bytes, pi_idx: bytes, pi_vals: bytes):
+        """The reference debugger's check (debugger.rs:95-205) against this prover's own selectors, with prove's
+        arguments: every failing row, ascending, as (row, identity family).  Empty means prove makes the proof.  Safe
+        beside proofs running on this prover."""
+        return debugger.query(self._unsatisfied_call(witnesses, pi_idx, pi_vals), self.n_constraints)[1]
+
+    def unsatisfied_report(self, witnesses: bytes, pi_idx: bytes, pi_vals: bytes):
+        """Debugger::unsatisfied_report (debugger.rs:221-236) for unsatisfied_constraints, without the call-site
+        clause; None when every constraint holds."""
+        n, first = debugger.query(self._unsatisfied_call(witnesses, pi_idx, pi_vals), 1)
+        return debugger.report(n, self.n_constraints, first)
 
     def __del__(self):
         try:
