@@ -461,18 +461,6 @@ __global__ void __launch_bounds__(256) k_poly_eval(EvalJobs jobs, uint4* partial
   const int j = blockIdx.y;
   cta_poly_eval(jobs.poly[j], jobs.len[j], jobs.point[j], partial + 2 * ((size_t)j * nblocks + blockIdx.x));
 }
-// The same for one set of points and several polynomials laid out with a fixed stride: job (y, z) evaluates
-// base + z * row_stride at point[y]; partial is [z][y][nblocks].
-struct EvalRows {
-  const uint4* base;
-  size_t row_stride;  // elements
-  unsigned len;
-  Fr point[16];
-};
-__global__ void __launch_bounds__(256) k_poly_eval_rows(EvalRows jobs, uint4* partial, unsigned nblocks) {
-  cta_poly_eval(jobs.base + 2 * (size_t)blockIdx.z * jobs.row_stride, jobs.len, jobs.point[blockIdx.y],
-                partial + 2 * (((size_t)blockIdx.z * gridDim.y + blockIdx.y) * nblocks + blockIdx.x));
-}
 // out[j] = sum_blk partial[j][blk] x_j^(2048 blk), x_j = pts.p[j mod npts]: Horner over the blocks
 struct EvalPoints {
   Fr p[16];
@@ -487,6 +475,140 @@ __global__ void k_sum_rows(const uint4* partial, unsigned nblocks, EvalPoints pt
 #pragma unroll 1
   for (unsigned b = nblocks; b-- > 0;) acc = acc * step + ld_fr_plain(partial, (size_t)j * nblocks + b);
   stg_fr(out, j, acc);
+}
+
+// Step 2 of the 4n-coset quotient evaluates polynomials on whole cosets s*H_8 (s = h: the points x_k; s = omega h:
+// omega x_k).  With y = s^8 and F_r(y) = sum_q c_{8q+r} y^q (r < 8),
+//   f(s w8^k) = sum_r w8^(rk) s^r F_r(y),
+// so a coefficient costs one product (a Horner step of its residue's fold) and the 8-point DFT runs once per
+// polynomial and coset.
+struct Coset8Consts {
+  Fr spow[2][8];   // s^r
+  Fr ypow[2][16];  // y^(2^i): lane (i < 5) and warp (5..7) weights, the Horner step y^256, block weights (i >= 10)
+  Fr w8pow[8];     // w8^k
+};
+// Jobs: row z of `rows` (row_len coefficients, stride row_stride) on coset c is job 2z + c, z < nrows; job 2 nrows
+// is `tail` (tail_len coefficients) on coset 0.  A job is split into blocks of kC8Block groups of eight
+// coefficients (the last block also takes the remainder); flat block index = job * row_blocks + block.
+constexpr unsigned kC8Per = 4;               // groups per thread in a full block
+constexpr unsigned kC8Block = 256 * kC8Per;  // = 2^10, so the block weight y^kC8Block is ypow[10]
+struct Coset8Jobs {
+  const uint4* rows;
+  size_t row_stride;
+  unsigned row_len, row_blocks;
+  int nrows;
+  const uint4* tail;
+  unsigned tail_len, tail_blocks;
+};
+PB_D Fr shfl_xor_fr(const Fr& a, int m) {
+  Fr r;
+#pragma unroll
+  for (int i = 0; i < 8; i++) r.v[i] = __shfl_xor_sync(0xffffffffu, a.v[i], m);
+  return r;
+}
+PB_D void sts_pair(uint4* s, const Fr& a) {
+  s[0] = make_uint4(a.v[0], a.v[1], a.v[2], a.v[3]);
+  s[1] = make_uint4(a.v[4], a.v[5], a.v[6], a.v[7]);
+}
+// Block b of a job: thread t folds the groups g = b kC8Block + t + 256 i below the block's end,
+//   acc_r = sum_i c_{8g+r} (y^256)^i,
+// then the CTA forms B_r = sum_t y^t acc_r (weights y^lane per thread, y^(32 warp) per warp) and writes it to
+// partial[8 blk + r]; the job's F_r is sum_b (y^kC8Block)^b B_r.
+__global__ void __launch_bounds__(256) k_coset8_eval(Coset8Jobs J, Coset8Consts C, uint4* partial) {
+  __shared__ uint4 sh[8][8][2];
+  const unsigned nrow_blk = 2 * J.nrows * J.row_blocks;
+  const uint4* poly;
+  unsigned len, b, nb;
+  int cs;
+  if (blockIdx.x < nrow_blk) {
+    const unsigned job = blockIdx.x / J.row_blocks;
+    b = blockIdx.x - job * J.row_blocks;
+    poly = J.rows + 2 * (size_t)(job >> 1) * J.row_stride;
+    len = J.row_len; nb = J.row_blocks; cs = job & 1;
+  } else {
+    b = blockIdx.x - nrow_blk;
+    poly = J.tail; len = J.tail_len; nb = J.tail_blocks; cs = 0;
+  }
+  const unsigned tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const size_t groups = (len + 7) / 8;
+  const size_t end = (b + 1 == nb) ? groups : (size_t)(b + 1) * kC8Block;
+  const size_t g0 = (size_t)b * kC8Block + tid;
+  const int top = g0 < end ? (int)((end - 1 - g0) / 256) : -1;  // this thread's last i
+  auto coef = [&](int i, int r) {
+    const size_t k = 8 * (g0 + 256 * (size_t)i) + r;
+    return k < len ? ld_fr_plain(poly, k) : Fr::zero();
+  };
+  Fr acc[8];
+#pragma unroll
+  for (int r = 0; r < 8; r++) acc[r] = top >= 0 ? coef(top, r) : Fr::zero();
+  const Fr step = C.ypow[cs][8];
+#pragma unroll 1
+  for (int i = top - 1; i >= 0; i--)
+#pragma unroll
+    for (int r = 0; r < 8; r++) acc[r] = acc[r] * step + coef(i, r);
+  Fr w = Fr::one();
+#pragma unroll
+  for (int k = 0; k < 5; k++)
+    if (lane >> k & 1) w = w * C.ypow[cs][k];
+#pragma unroll
+  for (int r = 0; r < 8; r++) {
+    Fr v = acc[r] * w;
+#pragma unroll
+    for (int m = 16; m > 0; m >>= 1) v = v + shfl_xor_fr(v, m);
+    if (lane == 0) sts_pair(sh[warp][r], v);
+  }
+  __syncthreads();
+  if (tid < 64) {  // warp tid >> 3, residue tid & 7
+    Fr v = lds_pair(sh[tid >> 3][tid & 7]);
+#pragma unroll
+    for (int k = 0; k < 3; k++)
+      if (tid >> (3 + k) & 1) v = v * C.ypow[cs][5 + k];
+    sts_pair(sh[tid >> 3][tid & 7], v);
+  }
+  __syncthreads();
+  if (tid < 8) {
+    Fr s = lds_pair(sh[0][tid]);
+#pragma unroll
+    for (int k = 1; k < 8; k++) s = s + lds_pair(sh[k][tid]);
+    stg_fr(partial, 8 * (size_t)blockIdx.x + tid, s);
+  }
+}
+// One CTA per job: thread (p, r) sums partial B_r of the blocks b = p mod 32 with weights Z^b, Z = y^kC8Block,
+// then out_k = sum_r w8^(rk) s^r F_r.  Row job 2z + c writes wpts[16 z + 8 c + k], the tail job ux[k].
+__global__ void __launch_bounds__(256) k_coset8_sum(Coset8Jobs J, Coset8Consts C, const uint4* partial, uint4* wpts, uint4* ux) {
+  __shared__ uint4 sh[8][8][2];
+  const unsigned job = blockIdx.x, nrj = 2 * J.nrows;
+  const unsigned nb = job < nrj ? J.row_blocks : J.tail_blocks;
+  const int cs = job < nrj ? (job & 1) : 0;
+  const unsigned tid = threadIdx.x, r = tid & 7, p = tid >> 3;
+  Fr w = Fr::one();
+#pragma unroll
+  for (int k = 0; k < 5; k++)
+    if (p >> k & 1) w = w * C.ypow[cs][10 + k];
+  Fr acc = Fr::zero();
+#pragma unroll 1
+  for (unsigned b = p; b < nb; b += 32) {
+    acc = acc + ld_fr_plain(partial, 8 * ((size_t)job * J.row_blocks + b) + r) * w;
+    w = w * C.ypow[cs][15];  // Z^32
+  }
+  acc = acc + shfl_xor_fr(acc, 8);
+  acc = acc + shfl_xor_fr(acc, 16);
+  if ((tid & 31) < 8) sts_pair(sh[tid >> 5][r], acc);
+  __syncthreads();
+  if (tid < 8) {  // thread r reads and rewrites column r only
+    Fr f = lds_pair(sh[0][r]);
+#pragma unroll
+    for (int k = 1; k < 8; k++) f = f + lds_pair(sh[k][r]);
+    sts_pair(sh[0][r], f * C.spow[cs][r]);
+  }
+  __syncthreads();
+  if (tid < 8) {
+    Fr out = lds_pair(sh[0][0]);
+#pragma unroll
+    for (int j = 1; j < 8; j++) out = out + lds_pair(sh[0][j]) * C.w8pow[(j * tid) & 7];
+    if (job < nrj) stg_fr(wpts, 16 * (job >> 1) + 8 * (job & 1) + tid, out);
+    else stg_fr(ux, tid, out);
+  }
 }
 
 // Step 3 + 4 of the 4n-coset quotient (see prove_dev): thread j < 8 computes
@@ -550,7 +672,7 @@ __global__ void k_scale_period8(uint4* p, size_t n, Period8 c) {
 }
 
 struct Quot4nConsts {
-  Fr xs[16];  // x_k = h w8^k (k < 8), then omega x_k
+  Coset8Consts c8;  // the cosets h H_8 (points x_k = h w8^k) and omega h H_8
   Quot4nFix fix;
 };
 
@@ -855,11 +977,14 @@ static int prover_build(pb200_prover* P, const uint8_t* label, size_t label_len,
     P->edwards_d = to_dev(pbh::edwards_d());
     const HFr g = to_host(ntt_coset_gen(false)), w8n = to_host(ntt_group_gen(log_n + 3, false));
     const HFr h = g * w8n, w8r = w8n.pow_u64(n), wn = to_host(ntt_group_gen(log_n, false)), g4n = g.pow_u64(4 * n);
-    HFr xs[16];
-    xs[0] = h;
-    for (int k = 1; k < 8; k++) xs[k] = xs[k - 1] * w8r;
-    for (int k = 0; k < 8; k++) xs[8 + k] = xs[k] * wn;
-    for (int k = 0; k < 16; k++) P->q4.xs[k] = to_dev(xs[k]);
+    const HFr shift[2] = {h, h * wn};
+    for (int c = 0; c < 2; c++) {
+      HFr p = HFr::one();
+      for (int r = 0; r < 8; r++, p = p * shift[c]) P->q4.c8.spow[c][r] = to_dev(p);
+      for (int i = 0; i < 16; i++, p = p.sqr()) P->q4.c8.ypow[c][i] = to_dev(p);  // p = s^8 first
+    }
+    HFr w8k = HFr::one();
+    for (int k = 0; k < 8; k++, w8k = w8k * w8r) P->q4.c8.w8pow[k] = to_dev(w8k);
     P->q4.fix.c = to_dev((g4n.dbl().neg()).inv());
     P->q4.fix.g4n = to_dev(g4n);
     const HFr h_inv = h.inv(), w8i = w8r.inv();
@@ -1402,38 +1527,29 @@ int prove_dev(const pb200_prover* P, int version, const uint64_t* d_wit, const u
       PB_LAUNCH(k_quotient_4n<2>, div_up(n4, 128), 128, 0, st, q);
     PB_TRY(ntt_run((const uint64_t*)quot, n4, (uint64_t*)tcoef, log_n + 2, 1, 1, 1, n4, n4, st, ar));
     // 2. t at the eight points x_k = h w8^k, h = g w_8n (indices 1 + n k of the 8n coset): the witness
-    //    polynomials by Horner at x_k and omega x_k, the prover key from its 8n tables.  The upper half
-    //    of w8 is free in this mode and holds the small arrays.
+    //    polynomials on the cosets h H_8 and omega h H_8 and u = tcoef on h H_8 (one fold per polynomial and
+    //    coset, k_coset8_eval), the prover key from its 8n tables.  The upper half of w8 is free in this mode and
+    //    holds the small arrays.
     uint4* wpts = w8 + 2 * 6 * n4;   // [6][16]
     uint4* tx = wpts + 2 * 96;       // t(x_k)
     uint4* ux = tx + 2 * 8;          // u(x_k)
-    uint4* part4 = ux + 2 * 8;       // partial sums of the evaluations
-    const unsigned blocks4 = div_up(n4, 2048);
+    uint4* part4 = ux + 2 * 8;       // [jobs][blocks][8] residue sums of the folds
     const Quot4nConsts& qc = P->q4;
     const int rows = n_pi ? 6 : 5;
     {
-      EvalRows er;
-      er.base = zp; er.row_stride = stride; er.len = (unsigned)n + 3;
-      for (int j = 0; j < 16; j++) er.point[j] = qc.xs[j];
-      EvalPoints ep;
-      for (int j = 0; j < 16; j++) ep.p[j] = qc.xs[j];
-      PB_LAUNCH(k_poly_eval_rows, dim3(eval_blocks, 16, rows), 256, 0, st, er, part4, eval_blocks);
-      PB_LAUNCH(k_sum_rows, 16 * rows, 32, 0, st, (const uint4*)part4, eval_blocks, ep, 16, wpts);
+      Coset8Jobs cj;
+      cj.rows = zp; cj.row_stride = stride; cj.row_len = (unsigned)n + 3; cj.nrows = rows;
+      cj.row_blocks = (unsigned)std::max<size_t>(1, div_up(n + 3, 8) / kC8Block);
+      cj.tail = tcoef; cj.tail_len = (unsigned)n4;
+      cj.tail_blocks = (unsigned)std::max<size_t>(1, (n4 / 8) / kC8Block);
+      PB_LAUNCH(k_coset8_eval, 2 * rows * cj.row_blocks + cj.tail_blocks, 256, 0, st, cj, qc.c8, part4);
+      PB_LAUNCH(k_coset8_sum, 2 * rows + 1, 256, 0, st, cj, qc.c8, (const uint4*)part4, wpts, ux);
     }
     if (!n_pi) PB_CUDA(cudaMemsetAsync(wpts + 2 * 16 * 5, 0, 16 * 32, st));
     QuotArgs qp = q;
     qp.w8 = wpts;
     qp.out = tx;
     PB_LAUNCH(k_quotient_pts, 1, 128, 0, st, qp);
-    {
-      EvalRows er;
-      er.base = tcoef; er.row_stride = 0; er.len = (unsigned)n4;
-      for (int j = 0; j < 16; j++) er.point[j] = qc.xs[j];
-      EvalPoints ep;
-      for (int j = 0; j < 16; j++) ep.p[j] = qc.xs[j];
-      PB_LAUNCH(k_poly_eval_rows, dim3(blocks4, 8, 1), 256, 0, st, er, part4, blocks4);
-      PB_LAUNCH(k_sum_rows, 8, 32, 0, st, (const uint4*)part4, blocks4, ep, 16, ux);
-    }
     // 3. t_hi(x_k) = (t(x_k) - u(x_k)) / (x_k^4n - g^4n), and x_k^4n = -g^4n for every k; the 8-point
     //    inverse DFT on h*H_8 gives its coefficients, the eighth of which must vanish (N divisible by Z_H:
     //    replaces the reference's len > 7n test, quotient_poly.rs:132-134);  4. t = (u - g^4n t_hi) + X^4n t_hi.
