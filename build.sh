@@ -8,7 +8,7 @@ OBJ=${PB200_OBJ:-build/obj}
 mkdir -p $OBJ
 NVFLAGS="-std=c++17 -O3 -lineinfo -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC -Xcompiler -O2 $*"
 pids=()
-for f in capi ntt msm prover ecntt verify debugger; do
+for f in capi ntt msm prover ecntt verify debugger pp; do
   nvcc $NVFLAGS -c -o $OBJ/$f.o $SRC/$f.cu &
   pids+=($!)
 done
@@ -16,5 +16,5 @@ g++ -std=c++17 -O2 -fPIC -c -o $OBJ/host_field.o $SRC/host_field.cpp
 g++ -std=c++17 -O2 -fPIC -c -o $OBJ/composer.o $SRC/composer.cpp
 g++ -std=c++17 -O2 -fPIC -c -o $OBJ/compress.o $SRC/compress.cpp
 for p in "${pids[@]}"; do wait $p; done
-nvcc -shared -o "$OUT" $OBJ/capi.o $OBJ/ntt.o $OBJ/msm.o $OBJ/prover.o $OBJ/ecntt.o $OBJ/verify.o $OBJ/debugger.o $OBJ/host_field.o $OBJ/composer.o $OBJ/compress.o
+nvcc -shared -o "$OUT" $OBJ/capi.o $OBJ/ntt.o $OBJ/msm.o $OBJ/prover.o $OBJ/ecntt.o $OBJ/verify.o $OBJ/debugger.o $OBJ/pp.o $OBJ/host_field.o $OBJ/composer.o $OBJ/compress.o
 echo "built $OUT"

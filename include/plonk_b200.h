@@ -32,6 +32,8 @@
  *                                    src/composer/circuit.rs:28-45, src/composer/compress.rs:136-240
  *   pb200_compressed_circuit_info / pb200_prover_from_compressed
  *                                    Compiler::compile_with_compressed   src/compiler.rs:84-112, compress.rs:242-461
+ *   pb200_pp_*                       one PublicParameters resident on the device, shared by the provers compiled from it
+ *                                    src/commitment_scheme/kzg10/srs.rs:61-196
  *   pb200_circuit_unsatisfied / pb200_prover_unsatisfied / pb200_identity_family
  *                                    Debugger::unsatisfied_constraints / unsatisfied_report   src/debugger.rs:31-236
  *   (Compiler::compile, src/compiler.rs:116-461, is pb200_prover_new, pb200_prover_commitments and pb200_verifier_new
@@ -89,6 +91,7 @@ typedef enum { PB200_PLONK_V1 = 1, PB200_PLONK_V2 = 2, PB200_PLONK_V3 = 3 } pb20
 typedef struct pb200_srs pb200_srs_t;
 typedef struct pb200_prover pb200_prover_t;
 typedef struct pb200_verifier pb200_verifier_t;
+typedef struct pb200_pp pb200_pp_t;
 
 /* ---- process / device ------------------------------------------------------------------- */
 /* Selects the device for this process.  Idempotent for the same device; ONE device per process: the
@@ -363,6 +366,51 @@ int pb200_compressed_circuit_info(const uint8_t* bytes, size_t len, size_t n_srs
  * prover writes.  A description without gates is PB200_ERR_INVALID_ARG ("empty circuit"), as for pb200_prover_new. */
 int pb200_prover_from_compressed(const uint8_t* label, size_t label_len, const uint8_t* bytes, size_t len,
                                  const uint8_t* srs_raw, size_t n_srs_points, pb200_prover_t** out);
+
+/* ---- device-resident public parameters (one PublicParameters for many Compiler::compile calls) -------------------- */
+/* A pb200_pp_t holds a PublicParameters on the device: its commit key as raw points in HBM and its opening key.  Provers
+ * made from it (pb200_prover_new_pp, _from_compressed_pp, _from_bytes_pp) prove, serialize and load exactly as those
+ * made from the same host points, but share the MSM tables derived from the key: the table of the trimmed key, one per
+ * trimmed point count next_pow2(constraints + 6) + 7, and the Lagrange-form table, one per domain size.  Each is built
+ * by the first prover that needs it (concurrent callers wait for that build; a failed build is retried by the next
+ * caller) and kept until pb200_pp_free.  Provers keep the tables they use, so they may outlive the pp.  Every call may
+ * run concurrently with the others on one pp except pb200_pp_free.  Too few points for a circuit is
+ * PB200_ERR_DEGREE_TOO_LARGE (Error::TruncatedDegreeTooLarge). */
+/* PublicParameters from raw points, as pb200_prover_new takes them (trusted, not validated), and OpeningKey::to_bytes,
+ * checked as pb200_opening_key_check does (PB200_ERR_POINT_MALFORMED). */
+int pb200_pp_new(const uint8_t* raw_points, size_t n_points, const uint8_t* opening_key, pb200_pp_t** out);
+/* PublicParameters::setup (srs.rs:61-100) with the commit key left on the device: arguments, errors and results as
+ * pb200_public_parameters_setup, and its argument errors come before any device work. */
+int pb200_pp_setup(size_t max_degree, const uint64_t* x, const uint64_t* g_scalar, const uint64_t* h_scalar, pb200_pp_t** out);
+/* checked = 1: PublicParameters::from_slice (srs.rs:163-178): the opening key, then 48-byte compressed points, decoded on
+ * the device straight into the pp with the on-curve and subgroup checks.  checked = 0: from_slice_unchecked (srs.rs:121-146)
+ * for PublicParameters::to_raw_var_bytes: the opening key, then the raw records, not validated.  The opening key is
+ * checked as pb200_opening_key_check does.  Too short (at most / fewer than PB200_OPENING_KEY_BYTES) is
+ * PB200_ERR_INVALID_ARG (NotEnoughBytes); a bad point, or compressed points that are not whole, PB200_ERR_POINT_MALFORMED. */
+int pb200_pp_from_slice(const uint8_t* bytes, size_t len, int checked, pb200_pp_t** out);
+/* The commit key's point count (PublicParameters::max_degree + 1); 0 for NULL. */
+size_t pb200_pp_points(const pb200_pp_t* pp);
+/* OpeningKey::to_bytes, PB200_OPENING_KEY_BYTES. */
+int pb200_pp_opening_key(const pb200_pp_t* pp, uint8_t* out_240);
+/* The commit key copied to the host: pb200_pp_points x 96 raw bytes. */
+int pb200_pp_raw_points(const pb200_pp_t* pp, uint8_t* out_raw);
+/* The derived tables the pp holds: how many trimmed-key and Lagrange-form tables, and their device bytes (any output may
+ * be NULL).  A table still being built is waited for. */
+int pb200_pp_tables(const pb200_pp_t* pp, size_t* n_monomial, size_t* n_lagrange, size_t* device_bytes);
+/* Frees the points and the cache's references to the tables; provers made from the pp are unaffected. */
+void pb200_pp_free(pb200_pp_t* pp);
+/* Compiler::compile's Prover::new (src/compiler.rs:116-461) from a pp: pb200_prover_new with pp's points. */
+int pb200_prover_new_pp(const pb200_pp_t* pp, const uint8_t* label, size_t label_len, size_t n_constraints,
+                        const uint64_t* selectors, const uint32_t* wires, size_t n_witnesses, pb200_prover_t** out);
+/* Compiler::compile_with_compressed's Prover (src/compiler.rs:84-112) from a pp: pb200_prover_from_compressed with pp's
+ * points, which also bound the decoding. */
+int pb200_prover_from_compressed_pp(const pb200_pp_t* pp, const uint8_t* label, size_t label_len,
+                                    const uint8_t* bytes, size_t len, pb200_prover_t** out);
+/* Prover::try_from_bytes (src/compiler/prover.rs:265-350) against a pp: pb200_prover_from_bytes, except that the
+ * serialized commit key must equal the pp's first points (one comparison on the device) in place of the per-point
+ * validation, so the prover carries over the pp's validation.  A key that is not such a prefix is PB200_ERR_INVALID_ARG. */
+int pb200_prover_from_bytes_pp(const pb200_pp_t* pp, const uint8_t* bytes, size_t len, const uint32_t* wires,
+                               size_t n_witnesses, pb200_prover_t** out);
 
 /* ---- verifier (Verifier::verify and verify_with_version; src/compiler/verifier.rs) ----------------------------- */
 /* Compiler::compile's Verifier half: the label, the circuit's constraint count, the 15 verifier-key commitments in

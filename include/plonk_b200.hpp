@@ -14,6 +14,9 @@
 //   plonk_b200::PlonkVersion       src/compiler.rs:22-42
 //   plonk_b200::PublicParameters   src/commitment_scheme/kzg10/srs.rs:61-196           setup, from_slice, from_slice_unchecked,
 //                                                                                      to_var_bytes, to_raw_var_bytes, max_degree
+//   plonk_b200::DevicePublicParameters  the same PublicParameters resident on the GPU, with the MSM tables of the
+//                                  provers compiled from it shared between them: setup, from_slice, from_slice_unchecked,
+//                                  from_host, to_host, tables
 //   plonk_b200::Compiler           src/compiler.rs:47-113, 116-461                     compile, compile_with_circuit,
 //                                                                                      compile_with_compressed
 //   plonk_b200::compress           src/composer/circuit.rs:28-45, src/composer/compress.rs:136-240   Circuit::compress
@@ -415,6 +418,8 @@ inline std::optional<std::string> unsatisfied_report(const Composer& composer) {
 // evaluations, so a V1 verdict is meaningful only for proofs made under the old rules.
 enum class PlonkVersion { V1 = PB200_PLONK_V1, V2 = PB200_PLONK_V2, V3 = PB200_PLONK_V3 };
 
+class DevicePublicParameters;
+
 class Prover {
  public:
   static constexpr size_t PROOF_SIZE = 1008;  // Proof::SIZE
@@ -423,6 +428,15 @@ class Prover {
     check(pb200_prover_new((const uint8_t*)label.data(), label.size(), c.n_constraints, c.selectors[0].data(), c.wires.data(),
                            c.n_witnesses, srs_raw, n_srs_points, &h_));
   }
+  // The same Prover with the commit-key tables of pp, shared with every other prover compiled from it
+  inline Prover(const std::string& label, const Circuit& c, const DevicePublicParameters& pp);
+  // try_from_bytes against pp: the serialized commit key must be a prefix of pp's points (else InvalidArgument), which
+  // stands in for the per-point validation; the tables are pp's
+  static inline std::unique_ptr<Prover> try_from_bytes(const DevicePublicParameters& pp, const uint8_t* bytes, size_t len,
+                                                       const std::vector<uint32_t>& wires, size_t n_witnesses);
+  // from_compressed with pp's points and tables
+  static inline std::unique_ptr<Prover> from_compressed(const std::string& label, const std::vector<uint8_t>& compressed,
+                                                        const DevicePublicParameters& pp, size_t n_witnesses);
   // Prover::try_from_bytes (prover.rs:265-350) for the bytes of Prover::to_bytes; the wiring of the circuit
   // (4 x constraints witness indices) is not part of that format and comes alongside
   static std::unique_ptr<Prover> try_from_bytes(const uint8_t* bytes, size_t len, const std::vector<uint32_t>& wires, size_t n_witnesses) {
@@ -712,6 +726,7 @@ class PublicParameters {
   size_t points() const { return raw_.size() / 96; }
 
  private:
+  friend class DevicePublicParameters;
   PublicParameters() = default;
   static void check_points(int rc) {
     if (rc == PB200_ERR_POINT_MALFORMED) throw Error(Error::PointMalformed, std::string("InvalidData: ") + pb200_last_error());
@@ -721,36 +736,133 @@ class PublicParameters {
   std::array<uint8_t, OPENING_KEY_SIZE> opening_key_{};
 };
 
+// PublicParameters resident on the GPU (pb200_pp_t): the commit key's points in HBM and the opening key.  Compiler
+// and Prover take it wherever they take PublicParameters; the provers made from it share the MSM tables derived from the
+// key (one per trimmed-key size and one per domain size), built once and kept until it is destroyed.  Those provers may
+// outlive it.  RAII and non-copyable.  Errors as PublicParameters'.
+class DevicePublicParameters {
+ public:
+  static constexpr size_t OPENING_KEY_SIZE = PB200_OPENING_KEY_BYTES;
+  struct Tables {
+    size_t monomial, lagrange, device_bytes;  // trimmed-key tables, Lagrange-form tables, their device bytes
+  };
+  // PublicParameters::setup with the commit key left on the device
+  static std::unique_ptr<DevicePublicParameters> setup(size_t max_degree, const BlsScalar& x, const BlsScalar& g_scalar,
+                                                       const BlsScalar& h_scalar) {
+    return make([&](pb200_pp_t** h) { return pb200_pp_setup(max_degree, x.data(), g_scalar.data(), h_scalar.data(), h); });
+  }
+  // PublicParameters::from_slice: every point decoded and validated on the device, straight into place
+  static std::unique_ptr<DevicePublicParameters> from_slice(const uint8_t* bytes, size_t len) {
+    if (len <= OPENING_KEY_SIZE) throw Error(Error::NotEnoughBytes, "NotEnoughBytes");
+    return make([&](pb200_pp_t** h) { return pb200_pp_from_slice(bytes, len, 1, h); });
+  }
+  // PublicParameters::from_slice_unchecked for to_raw_var_bytes
+  static std::unique_ptr<DevicePublicParameters> from_slice_unchecked(const uint8_t* bytes, size_t len) {
+    if (len < OPENING_KEY_SIZE) throw Error(Error::NotEnoughBytes, "NotEnoughBytes");
+    return make([&](pb200_pp_t** h) { return pb200_pp_from_slice(bytes, len, 0, h); });
+  }
+  // The same parameters uploaded once; the points are trusted as Prover's constructor trusts them
+  static std::unique_ptr<DevicePublicParameters> from_host(const PublicParameters& pp) {
+    return make([&](pb200_pp_t** h) { return pb200_pp_new(pp.raw_points().data(), pp.points(), pp.opening_key().data(), h); });
+  }
+  std::unique_ptr<PublicParameters> to_host() const {
+    std::unique_ptr<PublicParameters> pp(new PublicParameters());
+    pp->raw_.resize(96 * points());
+    check(pb200_pp_raw_points(h_, pp->raw_.data()));
+    pp->opening_key_ = opening_key_;
+    return pp;
+  }
+  Tables tables() const {
+    Tables t{0, 0, 0};
+    check(pb200_pp_tables(h_, &t.monomial, &t.lagrange, &t.device_bytes));
+    return t;
+  }
+  size_t points() const { return pb200_pp_points(h_); }
+  size_t max_degree() const { return points() - 1; }
+  const std::array<uint8_t, OPENING_KEY_SIZE>& opening_key() const { return opening_key_; }
+  const pb200_pp_t* handle() const { return h_; }
+  ~DevicePublicParameters() { pb200_pp_free(h_); }
+  DevicePublicParameters(const DevicePublicParameters&) = delete;
+  DevicePublicParameters& operator=(const DevicePublicParameters&) = delete;
+
+ private:
+  DevicePublicParameters() = default;
+  template <class F>
+  static std::unique_ptr<DevicePublicParameters> make(F&& construct) {
+    std::unique_ptr<DevicePublicParameters> pp(new DevicePublicParameters());
+    PublicParameters::check_points(construct(&pp->h_));
+    check(pb200_pp_opening_key(pp->h_, pp->opening_key_.data()));
+    return pp;
+  }
+  pb200_pp_t* h_ = nullptr;
+  std::array<uint8_t, OPENING_KEY_SIZE> opening_key_{};
+};
+
+inline Prover::Prover(const std::string& label, const Circuit& c, const DevicePublicParameters& pp)
+    : n_witnesses_(c.n_witnesses), n_constraints_(c.n_constraints) {
+  check(pb200_prover_new_pp(pp.handle(), (const uint8_t*)label.data(), label.size(), c.n_constraints, c.selectors[0].data(),
+                            c.wires.data(), c.n_witnesses, &h_));
+}
+inline std::unique_ptr<Prover> Prover::try_from_bytes(const DevicePublicParameters& pp, const uint8_t* bytes, size_t len,
+                                                      const std::vector<uint32_t>& wires, size_t n_witnesses) {
+  std::unique_ptr<Prover> p(new Prover());
+  p->n_witnesses_ = n_witnesses;
+  p->n_constraints_ = wires.size() / 4;
+  check(pb200_prover_from_bytes_pp(pp.handle(), bytes, len, wires.data(), n_witnesses, &p->h_));
+  return p;
+}
+inline std::unique_ptr<Prover> Prover::from_compressed(const std::string& label, const std::vector<uint8_t>& compressed,
+                                                       const DevicePublicParameters& pp, size_t n_witnesses) {
+  std::unique_ptr<Prover> p(new Prover());
+  p->n_witnesses_ = n_witnesses;
+  uint64_t described_witnesses = 0;
+  size_t n_labels = 0, n_pi = 0;
+  check(pb200_compressed_circuit_info(compressed.data(), compressed.size(), pp.points(), &p->n_constraints_, &described_witnesses,
+                                      &n_labels, &n_pi, nullptr));
+  check(pb200_prover_from_compressed_pp(pp.handle(), (const uint8_t*)label.data(), label.size(), compressed.data(),
+                                        compressed.size(), &p->h_));
+  return p;
+}
+
+namespace detail {
+inline Prover* new_prover(const std::string& label, const Circuit& c, const PublicParameters& pp) {
+  return new Prover(label, c, pp.raw_points().data(), pp.points());
+}
+inline Prover* new_prover(const std::string& label, const Circuit& c, const DevicePublicParameters& pp) { return new Prover(label, c, pp); }
+inline std::unique_ptr<Prover> compressed_prover(const std::string& label, const std::vector<uint8_t>& compressed,
+                                                 const PublicParameters& pp, size_t n_witnesses) {
+  return Prover::from_compressed(label, compressed, pp.raw_points().data(), pp.points(), n_witnesses);
+}
+inline std::unique_ptr<Prover> compressed_prover(const std::string& label, const std::vector<uint8_t>& compressed,
+                                                 const DevicePublicParameters& pp, size_t n_witnesses) {
+  return Prover::from_compressed(label, compressed, pp, n_witnesses);
+}
+}  // namespace detail
+
 // Compiler (compiler.rs): Prover::new, the prover's 15 verifier-key commitments and the Verifier over the same opening
 // key.  Public parameters too small for the circuit (pp.max_degree() < next_pow2(constraints + 6) + 6) throw
-// TruncatedDegreeTooLarge.
+// TruncatedDegreeTooLarge.  Every method takes PublicParameters or DevicePublicParameters; the provers compiled from one
+// DevicePublicParameters share its MSM tables.
 struct Compiler {
   using Pair = std::pair<std::unique_ptr<Prover>, std::unique_ptr<Verifier>>;
   // Compiler::compile for a filled composer
   static Pair compile(const PublicParameters& pp, const std::string& label, const Composer& composer) {
-    const Composer::Export e = composer.finish();
-    Pair out;
-    try {
-      out.first.reset(new Prover(label, circuit_of(e), pp.raw_points().data(), pp.points()));
-    } catch (const Error& err) {
-      if (err.kind == Error::PolynomialDegreeTooLarge) throw Error(Error::TruncatedDegreeTooLarge, err.what());
-      throw;
-    }
-    std::array<uint8_t, 15 * 48> comms;
-    check(pb200_prover_commitments(out.first->handle(), comms.data()));
-    out.second.reset(new Verifier(label, e.n_constraints, comms, pp.opening_key(), e.pi_idx));
-    return out;
+    return compile_as(pp, label, composer);
+  }
+  static Pair compile(const DevicePublicParameters& pp, const std::string& label, const Composer& composer) {
+    return compile_as(pp, label, composer);
   }
   // Compiler::compile_with_circuit: circuit(composer) fills a fresh Composer::initialized()
-  template <class F>
-  static Pair compile_with_circuit(const PublicParameters& pp, const std::string& label, F&& circuit) {
+  template <class PP, class F>
+  static Pair compile_with_circuit(const PP& pp, const std::string& label, F&& circuit) {
     Composer composer;
     circuit(composer);
     return compile(pp, label, composer);
   }
   // Compiler::compile_with_compressed (compiler.rs:84-112) for the bytes of compress(): the public parameters bound
   // the decoding.  Throws InvalidCompressedCircuit or BlsScalarMalformed for a description they refuse.
-  static Pair compile_with_compressed(const PublicParameters& pp, const std::string& label, const std::vector<uint8_t>& compressed) {
+  template <class PP>
+  static Pair compile_with_compressed(const PP& pp, const std::string& label, const std::vector<uint8_t>& compressed) {
     size_t n_constraints = 0, n_labels = 0, n_pi = 0;
     uint64_t n_witnesses = 0;
     check(pb200_compressed_circuit_info(compressed.data(), compressed.size(), pp.points(), &n_constraints, &n_witnesses, &n_labels,
@@ -760,10 +872,27 @@ struct Compiler {
       check(pb200_compressed_circuit_info(compressed.data(), compressed.size(), pp.points(), &n_constraints, &n_witnesses, &n_labels,
                                           &n_pi, pi_idx.data()));
     Pair out;
-    out.first = Prover::from_compressed(label, compressed, pp.raw_points().data(), pp.points(), (size_t)n_witnesses);
+    out.first = detail::compressed_prover(label, compressed, pp, (size_t)n_witnesses);
     std::array<uint8_t, 15 * 48> comms;
     check(pb200_prover_commitments(out.first->handle(), comms.data()));
     out.second.reset(new Verifier(label, n_constraints, comms, pp.opening_key(), pi_idx));
+    return out;
+  }
+
+ private:
+  template <class PP>
+  static Pair compile_as(const PP& pp, const std::string& label, const Composer& composer) {
+    const Composer::Export e = composer.finish();
+    Pair out;
+    try {
+      out.first.reset(detail::new_prover(label, circuit_of(e), pp));
+    } catch (const Error& err) {
+      if (err.kind == Error::PolynomialDegreeTooLarge) throw Error(Error::TruncatedDegreeTooLarge, err.what());
+      throw;
+    }
+    std::array<uint8_t, 15 * 48> comms;
+    check(pb200_prover_commitments(out.first->handle(), comms.data()));
+    out.second.reset(new Verifier(label, e.n_constraints, comms, pp.opening_key(), e.pi_idx));
     return out;
   }
 };

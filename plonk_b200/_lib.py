@@ -46,6 +46,8 @@ EXPORTS = [
     "pb200_g1_compress", "pb200_g1_compress_batch", "pb200_g1_decompress", "pb200_raw_commit_key_points", "pb200_commit_key_from_raw_var_bytes",
     "pb200_commit_key_to_raw_var_bytes", "pb200_prover_to_bytes", "pb200_g1_add_affine", "pb200_srs_setup_from_secret", "pb200_g1_lagrange_key",
     "pb200_public_parameters_setup", "pb200_opening_key_check",
+    "pb200_pp_new", "pb200_pp_setup", "pb200_pp_from_slice", "pb200_pp_points", "pb200_pp_opening_key", "pb200_pp_raw_points",
+    "pb200_pp_tables", "pb200_pp_free", "pb200_prover_new_pp", "pb200_prover_from_compressed_pp", "pb200_prover_from_bytes_pp",
     "pb200_circuit_compress", "pb200_compressed_circuit_info", "pb200_prover_from_compressed",
     "pb200_identity_family", "pb200_circuit_unsatisfied", "pb200_prover_unsatisfied",
     "pb200_profile_enable", "pb200_throughput_mode", "pb200_profile_read", "pb200_profile_read_sparse",
@@ -132,6 +134,19 @@ def lib() -> ctypes.CDLL:
         L.pb200_srs_setup_from_secret.argtypes = [c.c_void_p, c.c_void_p, c.c_size_t, c.c_void_p]
         L.pb200_public_parameters_setup.argtypes = [c.c_size_t, c.c_void_p, c.c_void_p, c.c_void_p, c.c_void_p, c.c_void_p]
         L.pb200_opening_key_check.argtypes = [c.c_void_p]
+        L.pb200_pp_new.argtypes = [c.c_void_p, c.c_size_t, c.c_void_p, c.POINTER(c.c_void_p)]
+        L.pb200_pp_setup.argtypes = [c.c_size_t, c.c_void_p, c.c_void_p, c.c_void_p, c.POINTER(c.c_void_p)]
+        L.pb200_pp_from_slice.argtypes = [c.c_void_p, c.c_size_t, c.c_int, c.POINTER(c.c_void_p)]
+        L.pb200_pp_points.argtypes = [c.c_void_p]
+        L.pb200_pp_points.restype = c.c_size_t
+        L.pb200_pp_opening_key.argtypes = [c.c_void_p, c.c_void_p]
+        L.pb200_pp_raw_points.argtypes = [c.c_void_p, c.c_void_p]
+        L.pb200_pp_tables.argtypes = [c.c_void_p, c.POINTER(c.c_size_t), c.POINTER(c.c_size_t), c.POINTER(c.c_size_t)]
+        L.pb200_pp_free.argtypes = [c.c_void_p]
+        L.pb200_pp_free.restype = None
+        L.pb200_prover_new_pp.argtypes = [c.c_void_p, c.c_void_p, c.c_size_t, c.c_size_t, c.c_void_p, c.c_void_p, c.c_size_t, c.POINTER(c.c_void_p)]
+        L.pb200_prover_from_compressed_pp.argtypes = [c.c_void_p, c.c_void_p, c.c_size_t, c.c_void_p, c.c_size_t, c.POINTER(c.c_void_p)]
+        L.pb200_prover_from_bytes_pp.argtypes = [c.c_void_p, c.c_void_p, c.c_size_t, c.c_void_p, c.c_size_t, c.POINTER(c.c_void_p)]
         L.pb200_circuit_compress.argtypes = [c.c_size_t, c.c_void_p, c.c_void_p, c.c_size_t, c.c_void_p, c.c_size_t, c.c_int, c.c_void_p,
                                              c.c_size_t, c.POINTER(c.c_size_t)]
         L.pb200_compressed_circuit_info.argtypes = [c.c_void_p, c.c_size_t, c.c_size_t, c.POINTER(c.c_size_t), c.POINTER(c.c_uint64),

@@ -4,11 +4,11 @@ opening key.  Circuit::compress (src/composer/circuit.rs:28-45) writes the descr
 from __future__ import annotations
 
 import ctypes
-from typing import Callable, Tuple
+from typing import Callable, Tuple, Union
 
 from ._lib import PB200_ERR_DEGREE_TOO_LARGE, PB200_ERR_INVALID_ARG, PB200_ERR_INVALID_COMPRESSED, PB200_ERR_SCALAR_MALFORMED, Pb200Error, check, lib
 from .prover import Prover, compressed_circuit_info
-from .srs import PublicParameters
+from .srs import DevicePublicParameters, PublicParameters
 from .verifier import Verifier
 
 
@@ -63,14 +63,29 @@ def compress(circuit: Callable, hades_optimization: bool = True) -> bytes:
     return compress_arrays(composer.arrays(), hades_optimization)
 
 
+Parameters = Union[PublicParameters, DevicePublicParameters]
+
+
+def _keys(pp: Parameters):
+    """What Prover takes for the commit key: the raw points of host parameters, or the device parameters themselves."""
+    return pp if isinstance(pp, DevicePublicParameters) else pp.raw_points
+
+
+def _points(pp: Parameters) -> int:
+    return pp.points() if isinstance(pp, DevicePublicParameters) else len(pp.raw_points) // 96
+
+
 class Compiler:
+    """Each method takes PublicParameters or DevicePublicParameters; the provers compiled from one
+    DevicePublicParameters share its MSM tables instead of building their own."""
+
     @staticmethod
-    def compile(pp: PublicParameters, label: bytes, composer) -> Tuple[Prover, Verifier]:
+    def compile(pp: Parameters, label: bytes, composer) -> Tuple[Prover, Verifier]:
         """Compiler::compile for a filled composer: anything with .arrays() (the Python Composer or the native gadget
         Composer).  Returns (Prover, Verifier)."""
         a = composer.arrays()
         try:
-            prover = Prover(label, a.constraints, a.selectors, a.wires, a.n_witnesses, pp.raw_points)
+            prover = Prover(label, a.constraints, a.selectors, a.wires, a.n_witnesses, _keys(pp))
         except Pb200Error as e:
             if e.code == PB200_ERR_DEGREE_TOO_LARGE:
                 raise TruncatedDegreeTooLarge("TruncatedDegreeTooLarge") from e
@@ -79,7 +94,7 @@ class Compiler:
         return prover, verifier
 
     @staticmethod
-    def compile_with_circuit(pp: PublicParameters, label: bytes, circuit: Callable) -> Tuple[Prover, Verifier]:
+    def compile_with_circuit(pp: Parameters, label: bytes, circuit: Callable) -> Tuple[Prover, Verifier]:
         """Compiler::compile_with_circuit: circuit(composer) fills a fresh native Composer.initialized()."""
         from .gadgets import Composer
 
@@ -88,12 +103,12 @@ class Compiler:
         return Compiler.compile(pp, label, composer)
 
     @staticmethod
-    def compile_with_compressed(pp: PublicParameters, label: bytes, compressed: bytes) -> Tuple[Prover, Verifier]:
+    def compile_with_compressed(pp: Parameters, label: bytes, compressed: bytes) -> Tuple[Prover, Verifier]:
         """Compiler::compile_with_compressed (compiler.rs:84-112): the Prover and Verifier of a description written by
         compress.  The public parameters bound the decoding; raises InvalidCompressedCircuit or BlsScalarMalformed for a
         description they reject.  The Prover's prove takes the re-run circuit's witness table."""
-        info = _compressed_errors(lambda: compressed_circuit_info(compressed, len(pp.raw_points) // 96))
-        prover = _compressed_errors(lambda: Prover.from_compressed(label, compressed, pp.raw_points, info))
+        info = _compressed_errors(lambda: compressed_circuit_info(compressed, _points(pp)))
+        prover = _compressed_errors(lambda: Prover.from_compressed(label, compressed, _keys(pp), info))
         n_constraints, _, _, _, pi_idx = info
         verifier = Verifier(label, n_constraints, prover.commitments(), pp.opening_key, pi_idx)
         return prover, verifier

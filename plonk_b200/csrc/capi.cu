@@ -131,6 +131,23 @@ void raw_commit_key_record(const uint8_t* raw96, uint8_t* rec97) {
   if (zero) memcpy(rec97 + 48, pbh::kFpMod.r1, 48);
   rec97[96] = zero ? 1 : 0;
 }
+
+// A draw of util::random_nonzero_bls_scalar: a canonical Montgomery residue (below r) that is not zero.
+static bool nonzero_canonical_scalar(const uint64_t* s) {
+  if (!(s[0] | s[1] | s[2] | s[3])) return false;
+  for (int k = 3; k >= 0; k--)
+    if (s[k] != pbh::kFrMod.p[k]) return s[k] < pbh::kFrMod.p[k];
+  return false;
+}
+
+int setup_args_check(size_t max_degree, const uint64_t* x, const uint64_t* g_scalar, const uint64_t* h_scalar) {
+  if (!x || !g_scalar || !h_scalar) return fail(PB200_ERR_INVALID_ARG, "null argument");
+  if (max_degree == 0) return fail(PB200_ERR_DEGREE_IS_ZERO, "DegreeIsZero");
+  if (max_degree > SIZE_MAX / 96 - 7) return fail(PB200_ERR_INVALID_ARG, "max_degree too large");
+  if (!nonzero_canonical_scalar(x) || !nonzero_canonical_scalar(g_scalar) || !nonzero_canonical_scalar(h_scalar))
+    return fail(PB200_ERR_INVALID_ARG, "a setup draw is zero or not a canonical scalar");
+  return 0;
+}
 }  // namespace pb
 
 using namespace pb;
@@ -380,21 +397,10 @@ int pb200_srs_setup_from_secret(const uint64_t* x, const uint64_t* g_scalar, siz
   return srs_setup(x, g_scalar, n_points, out_raw);
 }
 
-// A draw of util::random_nonzero_bls_scalar: a canonical Montgomery residue (below r) that is not zero.
-static bool nonzero_canonical_scalar(const uint64_t* s) {
-  if (!(s[0] | s[1] | s[2] | s[3])) return false;
-  for (int k = 3; k >= 0; k--)
-    if (s[k] != pbh::kFrMod.p[k]) return s[k] < pbh::kFrMod.p[k];
-  return false;
-}
-
 int pb200_public_parameters_setup(size_t max_degree, const uint64_t* x, const uint64_t* g_scalar, const uint64_t* h_scalar,
                                   uint8_t* out_raw_points, uint8_t* out_opening_key) {
-  if (!x || !g_scalar || !h_scalar || !out_raw_points || !out_opening_key) return fail(PB200_ERR_INVALID_ARG, "null argument");
-  if (max_degree == 0) return fail(PB200_ERR_DEGREE_IS_ZERO, "DegreeIsZero");
-  if (max_degree > SIZE_MAX / 96 - 7) return fail(PB200_ERR_INVALID_ARG, "max_degree too large");
-  if (!nonzero_canonical_scalar(x) || !nonzero_canonical_scalar(g_scalar) || !nonzero_canonical_scalar(h_scalar))
-    return fail(PB200_ERR_INVALID_ARG, "a setup draw is zero or not a canonical scalar");
+  if (!out_raw_points || !out_opening_key) return fail(PB200_ERR_INVALID_ARG, "null argument");
+  PB_TRY(setup_args_check(max_degree, x, g_scalar, h_scalar));
   PB_TRY(ensure_init());
   const size_t n = max_degree + 7;  // max_degree + ADDED_BLINDING_DEGREE + 1 powers (srs.rs:66-79)
   PB_TRY(srs_setup(x, g_scalar, n, out_raw_points));

@@ -1,8 +1,11 @@
 // The library's internal interface: every pb:: function and global that one translation unit defines and another uses.
 #pragma once
+#include <memory>
+
 #include "common.cuh"
 
 struct pb200_srs;  // a commit key on the device (msm.cu)
+struct pb200_pp;   // public parameters on the device (pp.cu)
 
 namespace pb {
 
@@ -37,6 +40,7 @@ size_t srs_len(const pb200_srs* s);
 int srs_window(const pb200_srs* s);
 void srs_free(pb200_srs* s);
 int srs_setup(const uint64_t* x_mont, const uint64_t* g_scalar_mont, size_t n, uint8_t* out_raw);
+int srs_setup_dev(const uint64_t* x_mont, const uint64_t* g_scalar_mont, size_t n, uint4* d_out);  // n x 96 bytes, synchronised
 int g1_decompress(const uint8_t* in, size_t n, int check_subgroup, uint8_t* out_raw);
 void g1_decompress_dev(const uint8_t* d_in, size_t n, uint4* d_out, unsigned* d_bad, cudaStream_t st);
 int g1_check_raw(const uint8_t* raw, size_t n);
@@ -62,7 +66,20 @@ int opening_key_g2(const uint64_t* x_mont, const uint64_t* h_scalar_mont, uint8_
 int unsatisfied_run(const uint4* sel, const uint4* wv, const uint4* pi, size_t n, size_t constraints, size_t cap, uint64_t* rows,
                     int32_t* families, size_t* n_unsatisfied, cudaStream_t st);
 
+// pp.cu: the MSM tables of one prover's commit key - the monomial table over its trimmed n_points and, for most
+// domains, the Lagrange-form table of the domain of 2^log_n - built from host points for this prover alone (key_tables)
+// or taken from the pp's cache (pp_key_tables, PB200_ERR_DEGREE_TOO_LARGE when n_points exceeds the pp's).
+struct KeyTables {
+  std::shared_ptr<pb200_srs> mono, lag;  // lag is null when the prover commits its wires with the monomial table
+};
+int key_tables(const uint8_t* raw, size_t n_points, int log_n, cudaStream_t st, KeyTables* out);
+int pp_key_tables(const pb200_pp* pp, size_t n_points, int log_n, cudaStream_t st, KeyTables* out);
+size_t pp_points(const pb200_pp* pp);
+// PB200_ERR_INVALID_ARG unless the n host raw points are the pp's first n
+int pp_check_prefix(const pb200_pp* pp, const uint8_t* raw, size_t n);
+
 // capi.cu
+int setup_args_check(size_t max_degree, const uint64_t* x, const uint64_t* g_scalar, const uint64_t* h_scalar);
 int raw_commit_key_parse(const uint8_t* bytes, size_t len, int checked, size_t* n_points, uint8_t* out_raw);
 void raw_commit_key_record(const uint8_t* raw96, uint8_t* rec97);
 

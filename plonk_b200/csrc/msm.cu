@@ -1744,7 +1744,7 @@ static int srs_gen_table(const uint4** out) {
   return 0;
 }
 
-int srs_setup(const uint64_t* x_mont, const uint64_t* g_scalar_mont, size_t n, uint8_t* out_raw) {
+int srs_setup_dev(const uint64_t* x_mont, const uint64_t* g_scalar_mont, size_t n, uint4* d_out) {
   const uint4* table = nullptr;
   PB_TRY(srs_gen_table(&table));
   cudaStream_t st = thread_stream();
@@ -1752,22 +1752,31 @@ int srs_setup(const uint64_t* x_mont, const uint64_t* g_scalar_mont, size_t n, u
   const size_t want_threads = (size_t)std::max(1u, num_sms()) * 1024;
   const unsigned run = (unsigned)std::min<size_t>(32, std::max<size_t>(1, div_up(n, want_threads)));
   const size_t threads = div_up(div_up(n, run), 128) * 128;
-  uint4 *d = nullptr, *scratch = nullptr;  // plain allocations: a large key's buffers do not stay in the stream pool
-  PB_CUDA(cudaMalloc((void**)&d, n * 96));
+  uint4* scratch = nullptr;  // a plain allocation: a large key's scratch does not stay in the stream pool
   cudaError_t e = cudaMalloc((void**)&scratch, (size_t)run * threads * 96);
   Fr x, gs;
   memcpy(x.v, x_mont, 32);
   memcpy(gs.v, g_scalar_mont, 32);
   if (e == cudaSuccess) {
-    PB_LAUNCH(k_srs_setup, threads / 128, 128, 0, st, d, n, x, gs, table, scratch, run);
+    PB_LAUNCH(k_srs_setup, threads / 128, 128, 0, st, d_out, n, x, gs, table, scratch, run);
     e = cudaGetLastError();
   }
-  if (e == cudaSuccess) e = cudaMemcpyAsync(out_raw, d, n * 96, cudaMemcpyDeviceToHost, st);
   if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-  cudaFree(d);
   cudaFree(scratch);
   PB_CUDA(e);
   return 0;
+}
+
+int srs_setup(const uint64_t* x_mont, const uint64_t* g_scalar_mont, size_t n, uint8_t* out_raw) {
+  uint4* d = nullptr;
+  PB_CUDA(cudaMalloc((void**)&d, n * 96));
+  int rc = srs_setup_dev(x_mont, g_scalar_mont, n, d);
+  if (rc == 0) {
+    const cudaError_t e = cudaMemcpy(out_raw, d, n * 96, cudaMemcpyDeviceToHost);
+    if (e != cudaSuccess) rc = fail(PB200_ERR_CUDA, "commit-key setup copy", cudaGetErrorString(e));
+  }
+  cudaFree(d);
+  return rc;
 }
 
 int g1_decompress(const uint8_t* in, size_t n, int check_subgroup, uint8_t* out_raw) {

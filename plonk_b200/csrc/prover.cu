@@ -691,6 +691,7 @@ struct pb200_prover {
   // (unless PB200_LAGRANGE=0) [L_0(x)]G .. [L_{n-1}(x)]G, then [1]G, [x]G, [x^n]G, [x^(n+1)]G - the wire polynomials
   // are committed through their values (short scalars) plus the two blinder terms
   pb200_srs* srs_lag = nullptr;
+  pb::KeyTables keys;  // owns srs and srs_lag: this prover's alone, or shared through a pb200_pp's cache
   uint32_t* d_wires = nullptr;  // [4][constraints]
   uint4* d_polys = nullptr;     // [15][n]
   uint4* d_key8 = nullptr;      // [15][8n]
@@ -790,19 +791,30 @@ struct LoadedProverKey {
   uint8_t comm[N_POLY][48];
 };
 
-// selectors / wires / n_witnesses: the circuit as pb200_prover_new takes it.  loaded: a key read by
-// pb200_prover_from_bytes.  comp: a compressed circuit (selectors unused, wires = comp's dense ids, n_witnesses = the
-// circuit's own witness count); its selector columns are expanded on the device.
+// The commit-key tables of a circuit of `constraints` gates, whose Prover::new trims the key to next_pow2(constraints +
+// 6) + 6 powers (compiler.rs:121-124, srs.rs:188-196): the circuit's own from the host points srs_raw, or the cache's of
+// pp.  n_srs is the point count the trimmed key must fit in.
+static int circuit_key_tables(size_t constraints, const pb200_pp* pp, const uint8_t* srs_raw, size_t n_srs, cudaStream_t st,
+                              KeyTables* out) {
+  size_t n_trim = 1;
+  while (n_trim < constraints + 6) n_trim <<= 1;
+  const size_t keep = n_trim + 6;
+  if (keep + 1 > n_srs) return fail(PB200_ERR_DEGREE_TOO_LARGE, "public parameters too small for this circuit (TruncatedDegreeTooLarge)");
+  int log_n = 0;
+  while (((size_t)1 << log_n) < constraints) log_n++;
+  if (log_n + 3 >= 32) return fail(PB200_ERR_INVALID_DOMAIN, "quotient domain too large");
+  return pp ? pp_key_tables(pp, keep + 1, log_n, st, out) : key_tables(srs_raw, keep + 1, log_n, st, out);
+}
+
+// selectors / wires / n_witnesses: the circuit as pb200_prover_new takes it.  keys: circuit_key_tables' for it.
+// loaded: a key read by pb200_prover_from_bytes.  comp: a compressed circuit (selectors unused, wires = comp's dense ids,
+// n_witnesses = the circuit's own witness count); its selector columns are expanded on the device.
 static int prover_build(pb200_prover* P, const uint8_t* label, size_t label_len, size_t constraints, const uint64_t* selectors,
-                        const uint32_t* wires, size_t n_witnesses, const uint8_t* srs_raw, size_t n_srs, cudaStream_t st,
+                        const uint32_t* wires, size_t n_witnesses, const KeyTables& keys, cudaStream_t st,
                         const LoadedProverKey* loaded = nullptr, const pbz::CompressedDescription* comp = nullptr) {
   P->label.assign(label, label + label_len);
   P->constraints = constraints;
   P->n_witnesses = n_witnesses;
-  size_t n_trim = 1;
-  while (n_trim < constraints + 6) n_trim <<= 1;  // compiler.rs:121-124
-  size_t keep = n_trim + 6;                       // srs.rs:188-196
-  if (keep + 1 > n_srs) return fail(PB200_ERR_DEGREE_TOO_LARGE, "public parameters too small for this circuit (TruncatedDegreeTooLarge)");
   size_t n = 1;
   int log_n = 0;
   while (n < constraints) {
@@ -812,35 +824,9 @@ static int prover_build(pb200_prover* P, const uint8_t* label, size_t label_len,
   P->n = n;
   P->n8 = 8 * n;
   P->log_n = log_n;
-  if (log_n + 3 >= 32) return fail(PB200_ERR_INVALID_DOMAIN, "quotient domain too large");
-  PB_TRY(srs_upload(srs_raw, keep + 1, &P->srs, 0));
-  {
-    static const bool lagrange_env = [] {
-      const char* e = getenv("PB200_LAGRANGE");
-      return !e || atoi(e) != 0;
-    }();
-    if (lagrange_env && n >= 2 && keep + 1 >= n + 2) {
-      uint4* comb = nullptr;  // n Lagrange points + 4 monomial ones
-      PB_CUDA(cudaMalloc((void**)&comb, (n + 4) * 96));
-      const uint4* mono = srs_points(P->srs);
-      int rc = lagrange_key_dev(mono, log_n, comb, st);
-      const size_t idx[4] = {0, 1, n, n + 1};
-      cudaError_t e = cudaSuccess;
-      for (int k = 0; k < 4 && e == cudaSuccess; k++)
-        e = cudaMemcpyAsync(comb + 6 * (n + k), mono + 6 * idx[k], 96, cudaMemcpyDeviceToDevice, st);
-      if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-      // Window of the Lagrange-form key.  Its scalars are witness VALUES - mostly zero or a single small digit -
-      // so the bucket reduction (~2.3 additions per bucket whatever the scalars) outweighs the accumulation
-      // unless the window is narrower than the monomial key's: PB200_LAG_C overrides the default.
-      int lag_c = std::min(12, msm_window_for(n + 4));
-      if (const char* env = getenv("PB200_LAG_C")) lag_c = atoi(env);
-      if (lag_c < 2 || lag_c > 20) lag_c = 0;
-      if (rc == 0 && e == cudaSuccess) rc = srs_from_device(comb, n + 4, &P->srs_lag, lag_c);
-      cudaFree(comb);
-      PB_TRY(rc);
-      PB_CUDA(e);
-    }
-  }
+  P->keys = keys;
+  P->srs = keys.mono.get();
+  P->srs_lag = keys.lag.get();
   const size_t n8 = P->n8;
   PB_CUDA(cudaMalloc((void**)&P->d_wires, 4 * constraints * 4));
   PB_CUDA(cudaMalloc((void**)&P->d_polys, (size_t)N_POLY * n * 32));
@@ -1015,11 +1001,16 @@ static int prover_build(pb200_prover* P, const uint8_t* label, size_t label_len,
   return 0;
 }
 
-int prover_new(const uint8_t* label, size_t label_len, size_t constraints, const uint64_t* selectors,
-               const uint32_t* wires, size_t n_witnesses, const uint8_t* srs_raw, size_t n_srs, pb200_prover** out) {
-  if (constraints == 0) return fail(PB200_ERR_INVALID_ARG, "empty circuit");
+// circuit_key_tables, then prover_build.  pp: the public parameters the tables come from, or null for tables of the
+// prover's own from the host points srs_raw.
+static int prover_make(const pb200_pp* pp, const uint8_t* srs_raw, size_t n_srs, const uint8_t* label, size_t label_len,
+                       size_t constraints, const uint64_t* selectors, const uint32_t* wires, size_t n_witnesses,
+                       const LoadedProverKey* loaded, const pbz::CompressedDescription* comp, pb200_prover** out) {
+  cudaStream_t st = thread_stream();
+  KeyTables keys;
+  PB_TRY(circuit_key_tables(constraints, pp, srs_raw, n_srs, st, &keys));
   pb200_prover* P = new pb200_prover();
-  const int rc = prover_build(P, label, label_len, constraints, selectors, wires, n_witnesses, srs_raw, n_srs, thread_stream());
+  const int rc = prover_build(P, label, label_len, constraints, selectors, wires, n_witnesses, keys, st, loaded, comp);
   if (rc != 0) {
     prover_free(P);  // releases whatever had been allocated; the error message is already set
     return rc;
@@ -1028,27 +1019,27 @@ int prover_new(const uint8_t* label, size_t label_len, size_t constraints, const
   return 0;
 }
 
+int prover_new(const pb200_pp* pp, const uint8_t* label, size_t label_len, size_t constraints, const uint64_t* selectors,
+               const uint32_t* wires, size_t n_witnesses, const uint8_t* srs_raw, size_t n_srs, pb200_prover** out) {
+  if (constraints == 0) return fail(PB200_ERR_INVALID_ARG, "empty circuit");
+  return prover_make(pp, srs_raw, n_srs, label, label_len, constraints, selectors, wires, n_witnesses, nullptr, nullptr, out);
+}
+
 // Compiler::compile_with_compressed's Prover (compiler.rs:84-112): the description decoded on the host, its selector
 // columns expanded on the device.
-int prover_from_compressed(const uint8_t* label, size_t label_len, const uint8_t* bytes, size_t len, const uint8_t* srs_raw,
-                           size_t n_srs, pb200_prover** out) {
+int prover_from_compressed(const pb200_pp* pp, const uint8_t* label, size_t label_len, const uint8_t* bytes, size_t len,
+                           const uint8_t* srs_raw, size_t n_srs, pb200_prover** out) {
   pbz::CompressedDescription d;
   PB_TRY(pbz::decode(bytes, len, n_srs, &d));
   if (d.gates() == 0) return fail(PB200_ERR_INVALID_ARG, "empty circuit");
-  pb200_prover* P = new pb200_prover();
-  const int rc = prover_build(P, label, label_len, d.gates(), nullptr, d.wires.data(), (size_t)d.witnesses, srs_raw, n_srs,
-                              thread_stream(), nullptr, &d);
-  if (rc != 0) {
-    prover_free(P);
-    return rc;
-  }
-  *out = P;
-  return 0;
+  return prover_make(pp, srs_raw, n_srs, label, label_len, d.gates(), nullptr, d.wires.data(), (size_t)d.witnesses, nullptr, &d, out);
 }
 
 // Prover::try_from_bytes (src/compiler/prover.rs:265-350); the layout is spelled out at pb200_prover_from_bytes
-// in include/plonk_b200.h.
-int prover_from_bytes(const uint8_t* bytes, size_t len, const uint32_t* wires, size_t n_witnesses, pb200_prover** out) {
+// in include/plonk_b200.h.  With a pp, the serialized commit key must be a prefix of the pp's points, which stands in
+// for the per-point validation, and the tables come from the pp's cache.
+int prover_from_bytes(const pb200_pp* pp, const uint8_t* bytes, size_t len, const uint32_t* wires, size_t n_witnesses,
+                      pb200_prover** out) {
   auto be64 = [](const uint8_t* p) {
     uint64_t v = 0;
     for (int i = 0; i < 8; i++) v = (v << 8) | p[i];
@@ -1108,15 +1099,8 @@ int prover_from_bytes(const uint8_t* bytes, size_t len, const uint32_t* wires, s
   PB_TRY(raw_commit_key_parse(ck, ck_len, 1, &n_pts, nullptr));
   std::vector<uint8_t> raw(n_pts * 96);
   PB_TRY(raw_commit_key_parse(ck, ck_len, 1, &n_pts, raw.data()));
-  PB_TRY(g1_check_raw(raw.data(), n_pts));
-  pb200_prover* P = new pb200_prover();
-  const int rc = prover_build(P, label, label_len, constraints, nullptr, wires, n_witnesses, raw.data(), n_pts, thread_stream(), &key);
-  if (rc != 0) {
-    prover_free(P);
-    return rc;
-  }
-  *out = P;
-  return 0;
+  PB_TRY(pp ? pp_check_prefix(pp, raw.data(), n_pts) : g1_check_raw(raw.data(), n_pts));
+  return prover_make(pp, raw.data(), n_pts, label, label_len, constraints, nullptr, wires, n_witnesses, &key, nullptr, out);
 }
 
 // Moves key material from HBM into the caller's (pageable) buffer without a second copy of the key on the device:
@@ -1312,8 +1296,6 @@ int prover_to_bytes(const pb200_prover* P, uint8_t* out, size_t cap, size_t* len
 
 void prover_free(pb200_prover* P) {
   if (!P) return;
-  if (P->srs) srs_free(P->srs);
-  if (P->srs_lag) srs_free(P->srs_lag);
   cudaFree(P->d_wires); cudaFree(P->d_polys); cudaFree(P->d_key8); cudaFree(P->d_linear8); cudaFree(P->d_l1_8); cudaFree(P->d_sigma);
   cudaFree(P->d_labels);
   for (char* w : P->ws_all) cudaFree(w);
@@ -1696,14 +1678,28 @@ int pb200_prover_new(const uint8_t* label, size_t label_len, size_t n_constraint
                      pb200_prover_t** out) {
   PB_TRY(ensure_init());
   if (!selectors || !wires || !srs_raw || !out) return fail(PB200_ERR_INVALID_ARG, "null argument");
-  return prover_new(label, label_len, n_constraints, selectors, wires, n_witnesses, srs_raw, n_srs_points, out);
+  return prover_new(nullptr, label, label_len, n_constraints, selectors, wires, n_witnesses, srs_raw, n_srs_points, out);
+}
+
+int pb200_prover_new_pp(const pb200_pp_t* pp, const uint8_t* label, size_t label_len, size_t n_constraints, const uint64_t* selectors,
+                        const uint32_t* wires, size_t n_witnesses, pb200_prover_t** out) {
+  PB_TRY(ensure_init());
+  if (!pp || !selectors || !wires || !out) return fail(PB200_ERR_INVALID_ARG, "null argument");
+  return prover_new(pp, label, label_len, n_constraints, selectors, wires, n_witnesses, nullptr, pp_points(pp), out);
 }
 
 int pb200_prover_from_compressed(const uint8_t* label, size_t label_len, const uint8_t* bytes, size_t len,
                                  const uint8_t* srs_raw, size_t n_srs_points, pb200_prover_t** out) {
   if ((!label && label_len) || !bytes || !srs_raw || !out) return fail(PB200_ERR_INVALID_ARG, "null argument");
   PB_TRY(ensure_init());
-  return prover_from_compressed(label, label_len, bytes, len, srs_raw, n_srs_points, out);
+  return prover_from_compressed(nullptr, label, label_len, bytes, len, srs_raw, n_srs_points, out);
+}
+
+int pb200_prover_from_compressed_pp(const pb200_pp_t* pp, const uint8_t* label, size_t label_len, const uint8_t* bytes, size_t len,
+                                    pb200_prover_t** out) {
+  if (!pp || (!label && label_len) || !bytes || !out) return fail(PB200_ERR_INVALID_ARG, "null argument");
+  PB_TRY(ensure_init());
+  return prover_from_compressed(pp, label, label_len, bytes, len, nullptr, pp_points(pp), out);
 }
 
 int pb200_throughput_mode(int on) {
@@ -1714,7 +1710,14 @@ int pb200_throughput_mode(int on) {
 int pb200_prover_from_bytes(const uint8_t* bytes, size_t len, const uint32_t* wires, size_t n_witnesses, pb200_prover_t** out) {
   PB_TRY(ensure_init());
   if (!bytes || !wires || !out) return fail(PB200_ERR_INVALID_ARG, "null argument");
-  return prover_from_bytes(bytes, len, wires, n_witnesses, out);
+  return prover_from_bytes(nullptr, bytes, len, wires, n_witnesses, out);
+}
+
+int pb200_prover_from_bytes_pp(const pb200_pp_t* pp, const uint8_t* bytes, size_t len, const uint32_t* wires, size_t n_witnesses,
+                               pb200_prover_t** out) {
+  PB_TRY(ensure_init());
+  if (!pp || !bytes || !wires || !out) return fail(PB200_ERR_INVALID_ARG, "null argument");
+  return prover_from_bytes(pp, bytes, len, wires, n_witnesses, out);
 }
 
 int pb200_prover_to_bytes(const pb200_prover_t* p, uint8_t* out, size_t cap, size_t* len) {

@@ -10,6 +10,7 @@ import ctypes
 
 from . import debugger
 from ._lib import PB200_ERR_UNSATISFIED, PB200_ERR_UNSUPPORTED_VERSION, Pb200Error, PlonkVersion, check, lib
+from .srs import DevicePublicParameters
 
 PROOF_BYTES = 1008
 
@@ -36,37 +37,51 @@ def compressed_circuit_info(compressed: bytes, n_srs_points: int):
 
 
 class Prover:
-    def __init__(self, label: bytes, n_constraints: int, selectors: bytes, wires: bytes, n_witnesses: int, srs_raw: bytes):
+    def __init__(self, label: bytes, n_constraints: int, selectors: bytes, wires: bytes, n_witnesses: int, srs_raw):
+        """srs_raw: the commit key as 96-byte raw points, or a DevicePublicParameters whose tables the prover shares."""
         assert len(selectors) == 11 * n_constraints * 32 and len(wires) == 4 * n_constraints * 4
         h = ctypes.c_void_p()
-        check(lib().pb200_prover_new(label, len(label), n_constraints, selectors, wires, n_witnesses, srs_raw,
-                                     len(srs_raw) // 96, ctypes.byref(h)))
+        if isinstance(srs_raw, DevicePublicParameters):
+            check(lib().pb200_prover_new_pp(srs_raw._h, label, len(label), n_constraints, selectors, wires, n_witnesses, ctypes.byref(h)))
+        else:
+            check(lib().pb200_prover_new(label, len(label), n_constraints, selectors, wires, n_witnesses, srs_raw,
+                                         len(srs_raw) // 96, ctypes.byref(h)))
         self._h = h
         self.n_constraints = n_constraints
         self.n_witnesses = n_witnesses
 
     @classmethod
-    def from_bytes(cls, prover_bytes: bytes, wires: bytes, n_witnesses: int) -> "Prover":
+    def from_bytes(cls, prover_bytes: bytes, wires: bytes, n_witnesses: int, pp: "DevicePublicParameters" = None) -> "Prover":
         """Prover::try_from_bytes (prover.rs:265-350) for the output of Prover::to_bytes; the circuit's wiring
-        (4 x constraints u32) is not part of that format and comes alongside."""
+        (4 x constraints u32) is not part of that format and comes alongside.  With pp, the serialized commit key must
+        be a prefix of pp's points (else a Pb200Error with PB200_ERR_INVALID_ARG) and the prover shares pp's tables."""
         self = cls.__new__(cls)
         h = ctypes.c_void_p()
-        check(lib().pb200_prover_from_bytes(prover_bytes, len(prover_bytes), wires, n_witnesses, ctypes.byref(h)))
+        if pp is None:
+            check(lib().pb200_prover_from_bytes(prover_bytes, len(prover_bytes), wires, n_witnesses, ctypes.byref(h)))
+        else:
+            check(lib().pb200_prover_from_bytes_pp(pp._h, prover_bytes, len(prover_bytes), wires, n_witnesses, ctypes.byref(h)))
         self._h = h
         self.n_constraints = len(wires) // 16
         self.n_witnesses = n_witnesses
         return self
 
     @classmethod
-    def from_compressed(cls, label: bytes, compressed: bytes, srs_raw: bytes, info=None) -> "Prover":
+    def from_compressed(cls, label: bytes, compressed: bytes, srs_raw, info=None) -> "Prover":
         """The Prover of Compiler::compile_with_compressed (compiler.rs:84-112): the selector columns are expanded on the
-        GPU from the description's tables.  prove takes the re-run circuit's witness table, as for any Prover.  info: what
-        compressed_circuit_info returned for these bytes and keys, if the caller has it already."""
-        n_constraints, n_witnesses, _, _, _ = info or compressed_circuit_info(compressed, len(srs_raw) // 96)
+        GPU from the description's tables.  prove takes the re-run circuit's witness table, as for any Prover.  srs_raw:
+        raw points or a DevicePublicParameters, as for Prover().  info: what compressed_circuit_info returned for these
+        bytes and keys, if the caller has it already."""
+        device = isinstance(srs_raw, DevicePublicParameters)
+        n_points = srs_raw.points() if device else len(srs_raw) // 96
+        n_constraints, n_witnesses, _, _, _ = info or compressed_circuit_info(compressed, n_points)
         self = cls.__new__(cls)
         h = ctypes.c_void_p()
-        check(lib().pb200_prover_from_compressed(label, len(label), compressed, len(compressed), srs_raw, len(srs_raw) // 96,
-                                                 ctypes.byref(h)))
+        if device:
+            check(lib().pb200_prover_from_compressed_pp(srs_raw._h, label, len(label), compressed, len(compressed), ctypes.byref(h)))
+        else:
+            check(lib().pb200_prover_from_compressed(label, len(label), compressed, len(compressed), srs_raw, n_points,
+                                                     ctypes.byref(h)))
         self._h = h
         self.n_constraints = n_constraints
         self.n_witnesses = n_witnesses

@@ -7,7 +7,7 @@ util::random_nonzero_bls_scalar that the reference makes (x, the G1 scalar, then
 from __future__ import annotations
 
 import ctypes
-from typing import Sequence
+from typing import NamedTuple, Sequence
 
 from ._lib import PB200_ERR_DEGREE_IS_ZERO, PB200_ERR_POINT_MALFORMED, Pb200Error, check, lib
 from . import kzg
@@ -98,3 +98,91 @@ class PublicParameters:
     def commit_key(self) -> kzg.CommitKey:
         """The commit key, uploaded to the GPU."""
         return kzg.CommitKey(self.raw_points)
+
+
+class PublicParameterTables(NamedTuple):
+    """The derived MSM tables a DevicePublicParameters holds: trimmed-key tables (one per trimmed point count),
+    Lagrange-form tables (one per domain size) and their device bytes."""
+
+    monomial: int
+    lagrange: int
+    device_bytes: int
+
+
+def _pp_call(call):
+    """A pb200_pp_* constructor: call(out) fills a handle; the errors PublicParameters raises are raised as such."""
+    h = ctypes.c_void_p()
+    try:
+        check(call(ctypes.byref(h)))
+    except Pb200Error as e:
+        if e.code == PB200_ERR_DEGREE_IS_ZERO:
+            raise DegreeIsZero("DegreeIsZero") from e
+        if e.code == PB200_ERR_POINT_MALFORMED:
+            raise PointMalformed(str(e)) from e
+        raise
+    return DevicePublicParameters(h)
+
+
+class DevicePublicParameters:
+    """One PublicParameters resident on the GPU (pb200_pp_t): the commit key's points in HBM and the opening key.  The
+    Compiler and Prover.from_bytes take it wherever they take a PublicParameters; the provers compiled from it share the
+    MSM tables derived from the key (one per trimmed-key size and one per domain size), built once and kept until this
+    object is freed.  Those provers may outlive it."""
+
+    def __init__(self, handle: ctypes.c_void_p):
+        self._h = handle
+        okey = ctypes.create_string_buffer(OPENING_KEY_BYTES)
+        check(lib().pb200_pp_opening_key(self._h, okey))
+        self.opening_key = okey.raw
+
+    @classmethod
+    def setup(cls, max_degree: int, draws: Sequence[bytes]) -> "DevicePublicParameters":
+        """PublicParameters.setup with the commit key left on the GPU: the same draws, points and errors."""
+        x, gs, hs = draws
+        assert len(x) == len(gs) == len(hs) == 32
+        return _pp_call(lambda out: lib().pb200_pp_setup(max_degree, x, gs, hs, out))
+
+    @classmethod
+    def from_slice(cls, data: bytes) -> "DevicePublicParameters":
+        """PublicParameters.from_slice, decoding and checking every point on the GPU straight into its place."""
+        if len(data) <= OPENING_KEY_BYTES:
+            raise NotEnoughBytes("NotEnoughBytes")
+        return _pp_call(lambda out: lib().pb200_pp_from_slice(data, len(data), 1, out))
+
+    @classmethod
+    def from_slice_unchecked(cls, data: bytes) -> "DevicePublicParameters":
+        """PublicParameters.from_slice_unchecked: the opening key checked, the raw commit-key records not."""
+        if len(data) < OPENING_KEY_BYTES:
+            raise NotEnoughBytes("NotEnoughBytes")
+        return _pp_call(lambda out: lib().pb200_pp_from_slice(data, len(data), 0, out))
+
+    @classmethod
+    def from_host(cls, pp: PublicParameters) -> "DevicePublicParameters":
+        """The same parameters uploaded once; the points are trusted as pb200_prover_new trusts them."""
+        n = len(pp.raw_points) // kzg.G1_RAW_BYTES
+        return _pp_call(lambda out: lib().pb200_pp_new(pp.raw_points, n, pp.opening_key, out))
+
+    def points(self) -> int:
+        return lib().pb200_pp_points(self._h)
+
+    def max_degree(self) -> int:
+        """PublicParameters::max_degree: one less than the commit key's point count."""
+        return self.points() - 1
+
+    def to_host(self) -> PublicParameters:
+        raw = ctypes.create_string_buffer(max(1, self.points()) * kzg.G1_RAW_BYTES)
+        check(lib().pb200_pp_raw_points(self._h, raw))
+        return PublicParameters(self.opening_key, raw.raw[: self.points() * kzg.G1_RAW_BYTES])
+
+    def tables(self) -> PublicParameterTables:
+        mono, lag, nbytes = ctypes.c_size_t(), ctypes.c_size_t(), ctypes.c_size_t()
+        check(lib().pb200_pp_tables(self._h, ctypes.byref(mono), ctypes.byref(lag), ctypes.byref(nbytes)))
+        return PublicParameterTables(mono.value, lag.value, nbytes.value)
+
+    def __del__(self):
+        try:
+            if getattr(self, "_h", None):
+                lib().pb200_pp_free(self._h)
+                self._h = None
+        except Exception:
+            pass
